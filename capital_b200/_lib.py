@@ -110,7 +110,7 @@ class Context:
         self._h = C.c_void_p()
         st = lib().capital_create(C.byref(self._h), C.byref(grid), device, C.c_void_p(stream or 0))
         if st != OK:
-            raise CapitalError(st, "capital_create failed (needs an sm_100 device; no CPU fallback exists)")
+            raise CapitalError(st, "capital_create failed (needs an sm_90 device; no CPU fallback exists)")
 
     def check(self, status: int):
         if status != OK:
@@ -185,7 +185,7 @@ class Context:
         return buf[:min(cap, n.value)].copy()
 
     def probe_dmma(self):
-        """(TFLOP/s, ms) of a register-resident DMMA.8x8x4 loop on every SM: the FP64 tensor-pipe ceiling of this device now."""
+        """(TFLOP/s, ms) of a register-resident DMMA.16x8x16 loop on every SM: the FP64 tensor-pipe ceiling of this device now."""
         tf, ms = C.c_double(), C.c_double()
         self.check(lib().capital_probe_dmma_f64(self._h, C.byref(tf), C.byref(ms)))
         return float(tf.value), float(ms.value)

@@ -5,7 +5,7 @@ model the kernel times.  Here one base-case policy exists (replicate-everything,
 cholinv/policy.h:160-224), the timing is the library's own CUDA-event bracket around `factor` (capital_last_factor_ms, max
 over ranks), and configurations whose multipliers clamp to the same base-case dimension (cholinv.hpp:15-18) are run once.
 
-    python -m torch.distributed.run --nproc-per-node 8 -m capital_b200.autotune 65536 1 0 1 -6 0 0 3 0 5
+    python -m torch.distributed.run --nproc-per-node 8 -m capital_b200.autotune 49152 1 0 1 -6 0 0 3 0 5
     (arguments as tune.cpp:164-176: num_rows rep_div complete_inv split bcMultiplier layout num_chunks num_iter compare [space_dim])
 
 `sweep()` is a pure function of a timing callback, so the selection logic is tested without a GPU (tests/test_autotune.py)."""

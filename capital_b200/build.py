@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (capital_b200/libcapital_b200.so) with nvcc for sm_100a, in-tree.
+"""Build the C-ABI shared library (capital_b200/libcapital_b200.so) with nvcc for sm_90a (H100), in-tree.
 
     python -m capital_b200.build [--force]
 
@@ -19,7 +19,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # products; an L1 line that survives from the previous use would be read back stale (seen as a handful of wrong 128-byte lines when
 # kernels of two streams overlap, i.e. when "kernel boundaries" no longer flush an SM's L1).  L2 is the coherence point for those
 # writes.  The hot loops do not depend on L1 (TMA -> shared memory, or explicit __ldcg), and the layout kernels are streaming.
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=hidden", "-Xptxas", "-v", "-Xptxas", "-dlcm=cg"]
 
 
@@ -50,7 +50,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 raise RuntimeError(f"nvcc failed on {src}")
     objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in SOURCES]
     if force or jobs or not os.path.exists(LIB):
-        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-ldl",
+        r = subprocess.run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-ldl",
                             "-Xcompiler", "-fPIC"], capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)

@@ -1,6 +1,6 @@
 // C ABI (include/capital_b200.h): context, grid helpers, generators, validators and the factor entry points.
 // Host orchestration only -- every flop and every byte of layout work runs in the kernels of gemm_tn.cu,
-// leaf.cu and layout.cu.  There is no CPU fallback: without a usable sm_100 device capital_create fails.
+// leaf.cu and layout.cu.  There is no CPU fallback: without a usable sm_90 device capital_create fails.
 #include "common.cuh"
 #include "dist.cuh"
 #include "peer.cuh"
@@ -263,8 +263,8 @@ int64_t capital_cholinv_bc_dimension(int64_t local_dim, int c, int d, int64_t bc
 
 // The deferred stream gets its own SM partition (a CUDA green context): all SMs but `reserve` of them.  Deferred GEMM tiles hold an
 // SM for up to ~1 ms and a running CTA cannot be preempted, so without a partition the latency-critical kernels of the chain
-// (8-CTA cluster base case, small products) wait that long for SMs although their stream has the higher priority: measured
-// 8034 us vs 144 us for ten 10-us cluster kernels behind a saturating low-priority kernel (profiles/r02a_probe_greenctx.log).
+// (8-CTA cluster base case, small products) wait that long for SMs although their stream has the higher priority (tools/probe_greenctx.cu
+// measures this).
 // The chain's streams stay in the primary context and may use every SM.
 static bool make_green_side_stream(capital_ctx* ctx, int reserve, int prio) {
   typedef CUresult (*fn_devget)(CUdevice*, int);
@@ -317,7 +317,7 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return CAPITAL_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return CAPITAL_ERR_CUDA;
-  if (prop.major != 10) return CAPITAL_ERR_CUDA;  // sm_100a binary only: no fallback path exists
+  if (prop.major != 9) return CAPITAL_ERR_CUDA;  // sm_90a binary only: no fallback path exists
   if (cudaSetDevice(device) != cudaSuccess) return CAPITAL_ERR_CUDA;
   capital_ctx* ctx = new capital_ctx();
   ctx->grid = *grid;
@@ -716,7 +716,7 @@ capital_status_t capital_blas_gemm_tn_f64(capital_ctx* ctx, int64_t m, int64_t n
   }
   return gemm_tn(ctx, ctx->stream, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags);
 }
-// EXPERIMENTAL (BASELINE config 5): the same product on the TF32 tensor cores (tcgen05 + TMEM), FP64 in and out
+// EXPERIMENTAL (BASELINE config 5): the same product on the TF32 tensor cores (wgmma), FP64 in and out
 capital_status_t capital_blas_gemm_tn_tf32(capital_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
                                            const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int passes) {
   if (!ctx || !A || !B || !C) return CAPITAL_ERR_INVALID;

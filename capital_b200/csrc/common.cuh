@@ -1,4 +1,4 @@
-// capital_b200 -- shared declarations for the CUDA translation units (sm_100a only).
+// capital_b200 -- shared declarations for the CUDA translation units (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -39,7 +39,7 @@ struct DeviceBuf {
 struct capital_ctx {
   capital_grid_t grid{};
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t stream = nullptr;   // main stream (caller's or owned)
   cudaStream_t side = nullptr;     // low-priority stream: deferred ("far") trailing updates, T^T products; lives in a green context
   void* green = nullptr;           // (CUgreenCtx) SM partition of the deferred stream, see make_green_side_stream (api.cu)
@@ -48,7 +48,7 @@ struct capital_ctx {
   cudaStream_t hi = nullptr;       // high-priority stream: the critical chain of the recursion
   cudaStream_t copy_in = nullptr, copy_out = nullptr;  // H2D / D2H streams of the host-pointer path
   // EXPERIMENTAL, off by default [env CAPITAL_ZC_OUT=1]: host outputs leave block by block through a kernel that stores straight
-  // into the pinned packed arrays (partial columns can leave as soon as they are final; see profiles/r01f_e2e_notes.md)
+  // into the pinned packed arrays (partial columns can leave as soon as they are final)
   cudaStream_t zc_out = nullptr;
   int zc_mode = 0, zc_ctas = 8, zc_depth = 3;  // [env CAPITAL_ZC_CTAS, CAPITAL_ZC_DEPTH]
   std::vector<cudaEvent_t> dep_pool;  // dependency events (timing disabled), recycled per factor call
@@ -76,9 +76,9 @@ struct capital_ctx {
   // per-launch timing of the dominant kernel (gemm_tn 128x128), off by default
   struct ProfRec { cudaEvent_t e0, e1; double flops; };
   bool profiling = false;
-  int64_t kchunk = 0;       // k-chunking of deferred GEMMs (env CAPITAL_KCHUNK); measured r01: 0 (off) is fastest, see profiles/r01c_notes.md
+  int64_t kchunk = 0;       // k-chunking of deferred GEMMs (env CAPITAL_KCHUNK); 0 = off
   int64_t far_min = 2048;   // trailing updates at least this large are split into near (critical) / far (deferred)   [env CAPITAL_FAR_MIN]
-  int64_t side_min = 1024;  // nodes whose left part is at least this large defer T^T to the low-priority stream      [env CAPITAL_SIDE_MIN]; swept in r01: 256 -> 68.9 ms, 1024 -> 67.0 ms
+  int64_t side_min = 1024;  // nodes whose left part is at least this large defer T^T to the low-priority stream      [env CAPITAL_SIDE_MIN]
   bool no_overlap = false;  // debug / measurement: run the recursion on one stream
   // EXPERIMENTAL, off by default (capital_set_trailing_precision): trailing updates A22 -= R12^T R12 on the TF32 tensor cores
   // (gemm_tf32.cu); 0 = FP64 DMMA, 1 = TF32, 3 = 3 x TF32 with split operands.  Products with k below tf32_min_k stay FP64.

@@ -198,7 +198,7 @@ struct Dist {
   bool bulk_class = true;    // node-entry pushes of A12 travel on their own push stream [env CAPITAL_DIST_BULK]
   bool flush_reads = true;   // read back from the partners between a storing GEMM and its flag [env CAPITAL_DIST_FLUSH_READS]
   bool pipeline = false;     // chunked products issue chunk j + 1 before adding up chunk j (hides the layers' skew) [env CAPITAL_DIST_PIPELINE];
-                             // protocol-checked, but off until it has a clean multi-GPU soak (profiles/r02c_coherence_bug_notes.md)
+                             // protocol-checked, but off until it has a clean multi-GPU soak
   // host-pointer callers: A arrives by column chunks on the copy-in stream; finished column ranges are packed and copied out while
   // the rest of the factorization runs
   std::vector<std::pair<int64_t, int>> in_chunks;  // (col_end, event)
@@ -288,8 +288,8 @@ struct Dist {
     }
     const int tli = ctx->tl_begin(strm(sid), 7, (double)rows, (double)cols, (double)dst_rank);
     // in pieces of at most 512 MiB (whole columns): a single peer copy of exactly 2 GiB -- the L x L operand of the n = 32768
-    // validator on the 2 x 2 x 2 grid -- was observed to let the flag that follows it overtake the tail of the data
-    // (profiles/r02c_coherence_bug_notes.md); smaller pieces also let several copy engines work on one push
+    // validator on the 2 x 2 x 2 grid -- was observed to let the flag that follows it overtake the tail of the data;
+    // smaller pieces also let several copy engines work on one push
     const int64_t cpp = std::max<int64_t>(1, ((int64_t)512 << 20) / (rows * 8));
     for (int64_t c0 = 0; c0 < cols; c0 += cpp) {
       const int64_t nc = std::min(cpp, cols - c0);

@@ -1,23 +1,23 @@
-// TF32 tensor-core (tcgen05 / TMEM) product for the MIXED-PRECISION trailing update of BASELINE config 5:
+// TF32 tensor-core (wgmma) product for the MIXED-PRECISION trailing update of BASELINE config 5:
 //     C[m x n] (FP64) = beta * C + alpha * sum_p A_p^T B_p        A_p: k x m, B_p: k x n  (FP32 copies of FP64 operands, col-major)
 //
-// EXPERIMENTAL -- OFF BY DEFAULT (capital_set_trailing_precision).  Written after the round's GPU budget was spent: it assembles for
-// sm_100a (SASS: UTCHMMA / UTMALDG / LDTM, profiles/r02_sass_tf32.md) but its first execution is whoever runs
-// tests/test_gpu_zz_late.py.  The default FP64 path never touches this file's kernels.
+// EXPERIMENTAL -- OFF BY DEFAULT (capital_set_trailing_precision).  The default FP64 path never touches this file's kernels.
 //
 // Why it exists: the reference has no float BLAS path (src/blas/interface.hpp:43-97 is double only); the FP64 trailing update
-// (summa::syrk, summa.hpp:143-145) is the one place of the hot path whose arithmetic a user may trade for speed, and the one place
-// where Blackwell's 5th-generation tensor cores apply (tcgen05 has no kind::f64).  The panel / base case, R12 and the inverse stay FP64.
+// (summa::syrk, summa.hpp:143-145) is the one place of the hot path whose arithmetic a user may trade for speed: Hopper's FP64
+// tensor rate is a fraction of its TF32 rate.  The panel / base case, R12 and the inverse stay FP64.
 //
-// B200 design.  Both operands are K-contiguous ("K-major" for UMMA), so a (128 rows x 32 k) FP32 tile is 128 rows of 128 bytes:
-// one TMA box per operand per stage (SWIZZLE_128B), consumed in place by tcgen05.mma.kind::tf32 (M = 128, N = 128, K = 8 per
-// instruction, four per stage) through shared-memory matrix descriptors; the 128 x 128 FP32 accumulator lives in TMEM (128 lanes x
-// 128 columns).  Warp roles: warp 0 lane 0 drives TMA, warp 1 lane 0 issues the MMAs and commits them to the stage's "empty"
-// mbarrier, warp 2 owns the TMEM allocation; afterwards all four warps read their 32 lanes with tcgen05.ld (32x32b.x16: thread =
-// accumulator row, 16 consecutive columns) and store FP64 -- for a fixed column the 32 lanes of a warp write 32 consecutive rows,
-// i.e. coalesced 256-byte segments of the column-major C.
+// H100 design.  Both operands are K-contiguous ("K-major" for wgmma, the only major-ness wgmma accepts for TF32), so a
+// (128 rows x 32 k) FP32 tile is 128 rows of 128 bytes: one TMA box per operand per stage (SWIZZLE_128B), consumed in place by
+// wgmma.mma_async.m64n128k8.f32.tf32.tf32 through shared-memory matrix descriptors (four per stage, K = 8 each).  Two consumer
+// warpgroups each own 64 rows of the 128 x 128 tile; a third warpgroup, of which one lane drives TMA, hands its registers to them
+// (setmaxnreg).  A consumer warpgroup releases a stage once its wgmma group has retired (wgmma.wait_group 0).
+// The tensor cores' FP32 accumulation truncates, so its error grows with the length of the contraction (measured on H100: a 3-pass
+// product at k = 8192 was off by 7e-6 of max |A|^T |B|, no better than the operand rounding it is meant to remove).  Each stage
+// therefore starts a fresh FP32 partial (scale-d = 0) that is added into FP64 register accumulators once the stage has retired:
+// only 32 products are ever summed in FP32.  The epilogue stores the FP64 accumulators (beta * C added) straight from registers.
 // passes = 3: every operand is split as x = hi + lo (both TF32-representable) and the product accumulates hi*hi + hi*lo + lo*hi in
-// the same TMEM tile: FP32-class accuracy at three times the tensor work (still an order of magnitude under the DMMA time).
+// the same accumulators: FP32-class accuracy at three times the tensor work.
 // Every mbarrier wait is bounded (2 s of %globaltimer): a protocol error ends the kernel with info = -3 instead of hanging the GPU.
 #include "common.cuh"
 #include <algorithm>
@@ -26,14 +26,13 @@ namespace {
 
 constexpr int TBM = 128, TBN = 128, TBK = 32;  // tile; TBK floats = one 128-byte swizzle row
 constexpr int TSTAGES = 6;
+constexpr int T_CWG = TBM / 64;                  // consumer warpgroups, 64 rows each
+constexpr int T_THREADS = (T_CWG + 1) * 128;     // + one producer warpgroup
+constexpr int T_REG_CONSUMER = 232, T_REG_PRODUCER = 40;  // 2 x 128 x 232 + 128 x 40 <= 64 K registers
 constexpr int T_A_BYTES = TBM * 128, T_B_BYTES = TBN * 128, T_STAGE_BYTES = T_A_BYTES + T_B_BYTES;
-constexpr int T_SMEM = TSTAGES * T_STAGE_BYTES + (2 * TSTAGES + 1) * 8 + 16 + 1024;
+constexpr int T_SMEM = TSTAGES * T_STAGE_BYTES + 2 * TSTAGES * 8 + 1024;
+static_assert(T_SMEM <= 227 * 1024, "shared memory of one H100 block");
 constexpr int T_PAIRS_MAX = 6;  // operand classes (<= 2) x passes (<= 3)
-constexpr uint32_t T_TMEM_COLS = 128;
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 @ [4,6), a_format / b_format TF32 = 2 @ [7,10) / [10,13),
-// a_major = b_major = K (0) @ 15 / 16, N >> 3 @ [17,23), M >> 4 @ [24,29)
-constexpr uint32_t T_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TBN >> 3) << 17) | ((uint32_t)(TBM >> 4) << 24);
-static_assert(T_IDESC == 0x08200910u, "instruction descriptor of tcgen05.mma.kind::tf32 128x128, K-major A and B");
 
 struct Tf32Maps {
   CUtensorMap a[T_PAIRS_MAX];
@@ -75,6 +74,9 @@ __device__ __forceinline__ bool mbar_wait_bounded(uint32_t bar, uint32_t parity,
     }
   }
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
@@ -84,27 +86,50 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor), K-major operand, 128-byte swizzle: start address >> 4 @ [0,14),
-// leading byte offset @ [16,30) (not used by the hardware for a swizzled K-major operand with one atom along K; 1 as
-// cute::UMMA::make_umma_desc<Major::K> sets it), stride byte offset = 8 rows x 128 B = 1024 (>> 4) @ [32,46), version 1 @ 46,
-// layout SWIZZLE_128B = 2 @ [61,64).  Tiles are 1024-byte aligned (base_offset 0).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// AND of `ok` over the 128 threads of a warpgroup (named barrier 1 + wg): every lane takes the same branch around the
+// .sync.aligned wgmma instructions even when the watchdog fires in some threads only
+__device__ __forceinline__ bool wg_all(bool ok, int wg) {
+  uint32_t r;
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "barrier.red.and.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(r)
+      : "r"((uint32_t)ok), "r"(1 + wg)
+      : "memory");
+  return r != 0;
+}
+// wgmma shared-memory matrix descriptor, K-major operand, 128-byte swizzle: start address >> 4 @ [0,14), leading byte offset @
+// [16,30) (unused for a swizzled K-major operand with one atom along K; 1 by convention), stride byte offset = 8 rows x 128 B =
+// 1024 (>> 4) @ [32,46), base offset 0 @ [49,52) (tiles are 1024-byte aligned), layout SWIZZLE_128B = 1 @ [62,64).
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
+}
+// d[64] = A (64 x 8, K-major in shared memory) * B (8 x 128, K-major in shared memory) [+ d when ACC], warpgroup-wide, asynchronous
+template <int ACC>
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "n"(ACC)
       : "memory");
 }
-// arrive on the mbarrier once every tcgen05.mma issued so far by this thread has completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-__global__ void __launch_bounds__(128, 1) gemm_tn_tf32_kernel(const __grid_constant__ Tf32Maps maps, const Tf32Params p) {
+__global__ void __launch_bounds__(T_THREADS, 1) gemm_tn_tf32_kernel(const __grid_constant__ Tf32Maps maps, const Tf32Params p) {
   extern __shared__ uint8_t smem_raw[];
   const int tm = blockIdx.x, tn = blockIdx.y;
   const int m0 = tm * TBM, n0 = tn * TBN;
@@ -118,97 +143,86 @@ __global__ void __launch_bounds__(128, 1) gemm_tn_tf32_kernel(const __grid_const
   const uint32_t smem_base = (raw_u32 + 1023u) & ~1023u;
   const uint32_t full0 = smem_base + TSTAGES * T_STAGE_BYTES;
   const uint32_t empty0 = full0 + TSTAGES * 8;
-  const uint32_t tfull = empty0 + TSTAGES * 8;
-  const uint32_t tmem_slot = tfull + 8;
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - raw_u32));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < TSTAGES; s++) {
       mbar_init(full0 + s * 8, 1);
-      mbar_init(empty0 + s * 8, 1);
+      mbar_init(empty0 + s * 8, T_CWG);
     }
-    mbar_init(tfull, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 2) {  // one warp allocates the accumulator's TMEM columns and lets other CTAs of the SM allocate too
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(T_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  if (warp == 0 && lane == 0) {
-    // ---------------- TMA producer ----------------
+  if (warp >= T_CWG * 4) {
+    // ---------------- TMA producer warpgroup: one lane issues, the group gives its registers to the consumers ----------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T_REG_PRODUCER));
+    if (warp != T_CWG * 4 || lane != 0) return;
     int it = 0;
-    bool alive = true;
-    for (int pr = 0; pr < p.npair && alive; pr++) {
+    for (int pr = 0; pr < p.npair; pr++) {
       const CUtensorMap* ma = &maps.a[pr];
       const CUtensorMap* mb = &maps.b[pr];
       for (int j = 0; j < nk; j++, it++) {
         const int s = it % TSTAGES;
         const uint32_t ph = (it / TSTAGES) & 1;
-        if (!mbar_wait_bounded(empty0 + s * 8, ph ^ 1, p.err)) { alive = false; break; }
+        if (!mbar_wait_bounded(empty0 + s * 8, ph ^ 1, p.err)) return;
         mbar_expect_tx(full0 + s * 8, T_STAGE_BYTES);
         tma_load_2d(smem_base + s * T_STAGE_BYTES, ma, full0 + s * 8, j * TBK, m0);
         tma_load_2d(smem_base + s * T_STAGE_BYTES + T_A_BYTES, mb, full0 + s * 8, j * TBK, n0);
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ---------------- MMA issuer: one thread on behalf of the CTA ----------------
-    for (int it = 0; it < niter; it++) {
-      const int s = it % TSTAGES;
-      const uint32_t ph = (it / TSTAGES) & 1;
-      if (!mbar_wait_bounded(full0 + s * 8, ph, p.err)) break;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint64_t da = umma_desc_k_sw128(smem_base + s * T_STAGE_BYTES);
-      const uint64_t db = umma_desc_k_sw128(smem_base + s * T_STAGE_BYTES + T_A_BYTES);
-#pragma unroll
-      for (int k8 = 0; k8 < TBK / 8; k8++)  // 8 floats = 32 bytes further along K inside the swizzle row: start address + 2 (>> 4)
-        umma_tf32(tmem_base, da + (uint64_t)(2 * k8), db + (uint64_t)(2 * k8), T_IDESC, (it > 0 || k8 > 0) ? 1u : 0u);
-      umma_commit(empty0 + s * 8);  // the stage is free again once these MMAs have read it
-    }
-    umma_commit(tfull);  // the accumulator is complete once everything issued above has retired
+    return;
   }
-  __syncwarp();
 
-  // ---------------- epilogue: all four warps, warp w reads TMEM lanes [32 w, 32 w + 32) ----------------
-  const bool have = mbar_wait_bounded(tfull, 0, p.err);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  __syncwarp();
-  const int row = m0 + warp * 32 + lane;
+  // ---------------- wgmma consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile ----------------
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T_REG_CONSUMER));
+  const int wg = warp >> 2;
+  float part[64];  // FP32 partial of one stage
+  double acc[64];  // FP64 sum of the partials
+#pragma unroll
+  for (int i = 0; i < 64; i++) acc[i] = 0.0;
+  bool have = true;
+  for (int it = 0; it < niter; it++) {
+    const int s = it % TSTAGES;
+    const uint32_t ph = (it / TSTAGES) & 1;
+    if (!wg_all(mbar_wait_bounded(full0 + s * 8, ph, p.err), wg)) { have = false; break; }
+    const uint64_t da = wgmma_desc_k_sw128(smem_base + s * T_STAGE_BYTES + wg * 64 * 128);
+    const uint64_t db = wgmma_desc_k_sw128(smem_base + s * T_STAGE_BYTES + T_A_BYTES);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    // 8 floats = 32 bytes further along K inside the swizzle row: start address + 2 (>> 4)
+    wgmma_m64n128k8_tf32<0>(part, da, db);
+#pragma unroll
+    for (int k8 = 1; k8 < TBK / 8; k8++) wgmma_m64n128k8_tf32<1>(part, da + (uint64_t)(2 * k8), db + (uint64_t)(2 * k8));
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    if ((threadIdx.x & 127) == 0) mbar_arrive(empty0 + s * 8);  // this warpgroup has finished reading the stage
+#pragma unroll
+    for (int i = 0; i < 64; i++) acc[i] += (double)part[i];
+  }
+  if (!have) return;
+
+  // ---------------- epilogue: fragment (j, i, e) of thread (warp w, lane l) is row 16 w + l / 4 + 8 i, column 8 j + 2 (l % 4) + e ----------------
   const double alpha = p.alpha, beta = p.beta;
   const bool upper_only = p.flags & CAPITAL_GEMM_C_UPPER;
-#pragma unroll 1
-  for (int c0 = 0; c0 < TBN; c0 += 16) {
-    if (n0 + c0 >= p.N) break;  // uniform over the CTA
-    __syncwarp();               // tcgen05.ld is .sync.aligned: the lanes that skipped the stores below rejoin here
-    uint32_t v[16];
-    const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    if (!have || row >= p.M) continue;
+  const int rbase = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-    for (int j = 0; j < 16; j++) {
-      const int col = n0 + c0 + j;
-      if (col >= p.N || (upper_only && row > col + p.noff)) continue;
-      double* cc = p.C + (long long)col * p.ldc + row;
-      double r = alpha * (double)__uint_as_float(v[j]);
-      if (beta != 0.0) r += beta * *cc;
-      *cc = r;
+  for (int j = 0; j < TBN / 8; j++) {
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+      const int col = n0 + j * 8 + 2 * (lane & 3) + e;
+      if (col >= p.N) continue;
+#pragma unroll
+      for (int i = 0; i < 2; i++) {
+        const int row = rbase + 8 * i;
+        if (row >= p.M || (upper_only && row > col + p.noff)) continue;
+        double* cc = p.C + (long long)col * p.ldc + row;
+        double r = alpha * acc[4 * j + 2 * i + e];
+        if (beta != 0.0) r += beta * *cc;
+        *cc = r;
+      }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(T_TMEM_COLS) : "memory");
 }
 
 // FP64 window (k x cols, ld) -> FP32 copies rounded to TF32 (cvt.rna): hi, and optionally lo = tf32(x - hi)
@@ -307,7 +321,7 @@ capital_status_t gemm_tn_tf32_x(capital_ctx* ctx, cudaStream_t st, int64_t m, in
   p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc; p.err = ctx->d_info;
   dim3 grid((unsigned)p.gm, (unsigned)p.gn, 1);
   const int tli = ctx->tl_begin(st, 9, (double)m, (double)n, (double)k);
-  gemm_tn_tf32_kernel<<<grid, 128, T_SMEM, st>>>(maps, p);
+  gemm_tn_tf32_kernel<<<grid, T_THREADS, T_SMEM, st>>>(maps, p);
   ctx->tl_end(st, tli);
   CAP_CUDA(cudaGetLastError());
   ctx->counters.kernel_launches++;

@@ -1,17 +1,19 @@
-// FP64 tensor-core GEMM for sm_100a:  C[m x n] = alpha * A^T B + beta * C   (A: k x m, B: k x n, col-major)
+// FP64 tensor-core GEMM for sm_90a:  C[m x n] = alpha * A^T B + beta * C   (A: k x m, B: k x n, col-major)
 //
 // This is the kernel behind every trailing update of the CholInv schedule -- the reference's
 // cblas_dgemm(T,N) in summa::syrk_internal (summa.hpp:143-145), cblas_dtrmm in summa::invoke
 // (summa.hpp:64,71) and the Gram products of cacqr (cacqr.hpp:15,95) -- with the triangular
 // structure the reference throws away (summa.hpp:115-116) turned into skipped k-tiles / output tiles.
 //
-// B200 design.  FP64 has no tcgen05 path (ptxas: "Unknown modifier .kind::f64"); the FP64 tensor pipe
-// is reached through mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4; measured 37.2 TFLOP/s = 64 FMA/clk/SM, see
-// profiles/r01_fp64_pipe_ceilings.log).  Both operands are K-contiguous, so a (rows x 16 k) tile is one
+// H100 design.  wgmma has no FP64 form; the FP64 tensor pipe is reached through mma.sync.m16n8k16.f64
+// (SASS DMMA.16x8x16, which sm_90 adds: on an H100 SXM at 700 W it delivers twice the rate of DMMA.8x8x4, measured
+// 66 vs 33 TFLOP/s in the register-resident loop below; the bench measures the ceiling in each run, capital_probe_dmma_f64).
+// Both operands are K-contiguous, so a (rows x 16 k) tile is one
 // 128-byte row per matrix column: TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) stages it with one
 // instruction per operand per stage from a dedicated producer warp; consumers wait on mbarriers (no
-// __syncthreads in the main loop).  Inside a 16-wide k tile the four DMMAs use the k permutation
-// {4q+j}: lane q then owns 32 contiguous bytes of every row, read as two conflict-free LDS.128
+// __syncthreads in the main loop).  One 16-wide k tile is one DMMA.16x8x16 per 16 x 8 output fragment; its
+// logical k index q + 4c is mapped to the stored k index 4q + c (the same permutation for A and B): lane q
+// then owns 32 contiguous bytes of every row, read as two conflict-free LDS.128
 // (the 128B swizzle XORs the 16B chunk index with row%8, so the 8 lanes of a quarter-warp -- two rows x
 // four q -- hit 8 distinct chunks).  Out-of-range rows/columns are zero-filled by TMA, so ragged M/N/K
 // need no predicates in the main loop.
@@ -74,14 +76,20 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+// D (16 x 8) += A (16 x 16) B (16 x 8), lane (g = lane / 4, q = lane % 4): a[i] = A[g + 8 (i % 2)][q + 4 (i / 2)],
+// b[i] = B[q + 4 i][g], {c0, c1} = D[g][2q, 2q + 1], {c2, c3} = D[g + 8][2q, 2q + 1]
+__device__ __forceinline__ void dmma16816(double& c0, double& c1, double& c2, double& c3, const double2 (&a0)[2], const double2 (&a1)[2],
+                                          const double2 (&b)[2]) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a0[0].x), "d"(a1[0].x), "d"(a0[0].y), "d"(a1[0].y), "d"(a0[1].x), "d"(a1[1].x), "d"(a0[1].y), "d"(a1[1].y),
+        "d"(b[0].x), "d"(b[0].y), "d"(b[1].x), "d"(b[1].y));
 }
 
 constexpr int BK = 16;  // doubles per k tile = one 128-byte swizzle row
 
 // Warp roles: NCW consumer warps (whole warpgroups) + one producer warpgroup of which a single lane drives TMA.
-// Registers are allocated per warpgroup on sm_100, so a 9th warp would be charged as four anyway; with RC > 0 the
+// Registers are allocated per warpgroup on sm_90, so a 9th warp would be charged as four anyway; with RC > 0 the
 // producer group hands its registers to the consumers (setmaxnreg), which is what lets a 64x32 warp tile
 // (128 accumulator registers) live without spills.
 // XMODE: 0 = plain product; 1 / 2 = depth exchange fused into the epilogue (GemmXDev in common.cuh).
@@ -90,6 +98,7 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
     gemm_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
   constexpr int NWM = BM / WM, NWN = BN / WN, NCW = NWM * NWN;
   constexpr int FM = WM / 8, FN = WN / 8;
+  static_assert(FM % 2 == 0, "DMMA.16x8x16 fragments pair the 8-row blocks of a warp tile");
   constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, STAGE_BYTES = A_BYTES + B_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
@@ -188,21 +197,31 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
     const uint32_t ph = (it / STAGES) & 1;
     mbar_wait(full0 + s * 8, ph);
     const uint8_t* st = smem + s * STAGE_BYTES;
+    // stored k 4q .. 4q + 3 of row g of every 8-row block: chunk swz[0] holds 4q, 4q + 1, chunk swz[1] holds 4q + 2, 4q + 3.
+    // With the producer's registers (RC > 0) the B fragments of the whole warp tile stay live across the A fragments (half the
+    // shared-memory reads); without them they are re-read per 16-row fragment, which keeps the small tile's register count down.
+    constexpr bool PRELOAD_B = RC > 0;
+    double2 bf[FN][2];
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      double2 af[FM], bf[FN];
+    for (int j = 0; j < FN; j++)
 #pragma unroll
-      for (int i = 0; i < FM; i++) af[i] = *reinterpret_cast<const double2*>(st + a_row_off + i * 1024 + swz[h]);
+      for (int h = 0; h < 2; h++)
+        if (PRELOAD_B) bf[j][h] = *reinterpret_cast<const double2*>(st + b_row_off + j * 1024 + swz[h]);
 #pragma unroll
-      for (int j = 0; j < FN; j++) bf[j] = *reinterpret_cast<const double2*>(st + b_row_off + j * 1024 + swz[h]);
+    for (int i = 0; i < FM; i += 2) {
+      double2 a0[2], a1[2];  // rows g and g + 8 of the 16-row fragment
 #pragma unroll
-      for (int i = 0; i < FM; i++)
+      for (int h = 0; h < 2; h++) {
+        a0[h] = *reinterpret_cast<const double2*>(st + a_row_off + i * 1024 + swz[h]);
+        a1[h] = *reinterpret_cast<const double2*>(st + a_row_off + (i + 1) * 1024 + swz[h]);
+      }
 #pragma unroll
-        for (int j = 0; j < FN; j++) dmma884(acc[i][j][0], acc[i][j][1], af[i].x, bf[j].x);
+      for (int j = 0; j < FN; j++) {
+        if (!PRELOAD_B)
 #pragma unroll
-      for (int i = 0; i < FM; i++)
-#pragma unroll
-        for (int j = 0; j < FN; j++) dmma884(acc[i][j][0], acc[i][j][1], af[i].y, bf[j].y);
+          for (int h = 0; h < 2; h++) bf[j][h] = *reinterpret_cast<const double2*>(st + b_row_off + j * 1024 + swz[h]);
+        dmma16816(acc[i][j][0], acc[i][j][1], acc[i + 1][j][0], acc[i + 1][j][1], a0, a1, bf[j]);
+      }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(empty0 + s * 8);
@@ -253,7 +272,7 @@ struct GemmCfg {
   static constexpr auto kernel() { return gemm_tn_kernel<BM, BN, WM, WN, STAGES, MINB, RC, RP, XMODE>; }
 };
 using CfgBig = GemmCfg<128, 128, 64, 32, 5, 1, 232, 40>;   // 8 consumer warps + producer group, 1 CTA / SM
-using CfgSmall = GemmCfg<64, 64, 32, 32, 6, 2, 0, 0>;       // 4 consumer warps + producer group, 2 CTAs / SM
+using CfgSmall = GemmCfg<64, 64, 32, 32, 6, 1, 0, 0>;       // 4 consumer warps + producer group (a 2-CTA/SM register cap spills the DMMA.16x8x16 fragments)
 
 capital_status_t make_map(capital_ctx* ctx, CUtensorMap* map, const double* base, int64_t rows, int64_t cols, int64_t ld,
                           int box_rows_k, int box_cols) {
@@ -335,26 +354,27 @@ capital_status_t launch(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n,
 }  // namespace
 
 // ---- FP64 tensor-pipe ceiling, measured in place ------------------------------------------------------------------
-// Register-resident DMMA.8x8x4 loop (8 independent accumulator pairs per warp, 8 warps per SM): what the tensor pipe delivers with
-// no memory traffic at all.  bench.py runs it next to the timed steps so that `roofline.peak` is a number of THIS device at THIS
+// Register-resident DMMA.16x8x16 loop (the instruction of gemm_tn_kernel; 8 independent accumulator sets per warp, 8 warps per SM):
+// what the tensor pipe delivers with no memory traffic at all.  bench.py runs it next to the timed steps so that `roofline.peak` is a number of THIS device at THIS
 // clock, not a constant from a file.
 __global__ void __launch_bounds__(256) dmma_peak_kernel(double* out, int iters, double s) {
-  double c[8][2];
+  double c[8][4];
 #pragma unroll
-  for (int i = 0; i < 8; i++) { c[i][0] = 0.0; c[i][1] = 0.0; }
+  for (int i = 0; i < 8; i++) c[i][0] = c[i][1] = c[i][2] = c[i][3] = 0.0;
   const double a = s + threadIdx.x * 1e-6, b = 1.0 - s;
   for (int it = 0; it < iters; it++) {
 #pragma unroll
     for (int i = 0; i < 8; i++)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[i][0]), "+d"(c[i][1]) : "d"(a), "d"(b));
+      asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%4,%4,%4,%4,%4,%4,%4}, {%5,%5,%5,%5}, {%0,%1,%2,%3};"
+                   : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(b));
   }
   double r = 0.0;
 #pragma unroll
-  for (int i = 0; i < 8; i++) r += c[i][0] + c[i][1];
+  for (int i = 0; i < 8; i++) r += c[i][0] + c[i][1] + c[i][2] + c[i][3];
   if (r == 123.456) out[0] = r;
 }
 capital_status_t gemm_probe_dmma(capital_ctx* ctx, double* tflops, double* ms_out) {
-  const int iters = 100000, blocks = ctx->num_sms;
+  const int iters = 25000, blocks = ctx->num_sms;
   cudaStream_t st = ctx->stream;
   dmma_peak_kernel<<<blocks, 256, 0, st>>>(ctx->d_scalars + 8, iters / 10, 0.5);  // warm-up
   CAP_CUDA(cudaEventRecord(ctx->ev_start, st));
@@ -363,7 +383,7 @@ capital_status_t gemm_probe_dmma(capital_ctx* ctx, double* tflops, double* ms_ou
   CAP_CUDA(cudaStreamSynchronize(st));
   float ms = 0;
   CAP_CUDA(cudaEventElapsedTime(&ms, ctx->ev_start, ctx->ev_stop));
-  const double flops = 2.0 * 256.0 * 8.0 * (double)iters * 8.0 * (double)blocks;  // 8x8x4 MACs x 8 accumulators x 8 warps x blocks
+  const double flops = 2.0 * 2048.0 * 8.0 * (double)iters * 8.0 * (double)blocks;  // 16x8x16 MACs x 8 accumulators x 8 warps x blocks
   *tflops = flops / (ms * 1e-3) / 1e12;
   *ms_out = ms;
   return CAPITAL_OK;
@@ -399,8 +419,8 @@ __global__ void splitk_reduce_kernel(long long rows, long long cols, const doubl
 
 // Split-K variant for short-and-fat products (the tall-skinny Gram matrix, cacqr.hpp:15): C = alpha A^T B with the k range cut
 // into chunks, one CTA per (tile, chunk); the partial tiles go to a workspace and are added up in chunk order by a second kernel
-// (deterministic: the same bits on every run and on every rank).  128 x 128 tiles when the output has them: 3 upper tiles x 49
-// chunks fill the 148 SMs for a 256 x 256 Gram matrix.
+// (deterministic: the same bits on every run and on every rank).  128 x 128 tiles when the output has them: 3 upper tiles x 44
+// chunks fill the 132 SMs of an H100 for a 256 x 256 Gram matrix.
 capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags) {
   if (m <= 0 || n <= 0 || k <= 0) return CAPITAL_OK;

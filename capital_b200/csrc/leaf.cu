@@ -8,7 +8,7 @@
 //                    64-wide panels -- diagonal block by the leaf routine, row panel and trailing update as 64x64x64
 //                    DMMA tile products spread over the cluster, hardware cluster barriers between phases -- followed
 //                    by the blocked triangular inverse.  One launch replaces ~60 latency-bound launches of the
-//                    recursion below 512 (r01a profile: leaves + small GEMMs were 37% of the step).
+//                    recursion below 512, where leaves and small GEMMs are latency-bound.
 // The critical path of a leaf is the pivot chain (64 dependent rsqrt + rank-1 updates), so the leaf keeps all
 // 256 threads on a fixed 16x16 grid (no index division), scales the pivot row with two warps, and uses one
 // rsqrt per pivot instead of a sqrt and a divide.
@@ -235,9 +235,9 @@ __device__ __forceinline__ void tile_store_from_rowmajor(double* __restrict__ ds
 
 // ---- fast 64 x 64 leaf: two warp-resident 32 x 32 factor+invert steps glued by DMMA products ------------------
 // The pivot chain is the critical path of the whole factorization (16384 dependent pivots at n = 16384).  A block-wide
-// formulation pays two __syncthreads and several shared-memory round trips per pivot (~1200 cycles measured); here
+// formulation pays two __syncthreads and several shared-memory round trips per pivot; here
 // a single warp holds a 32 x 32 block in registers (lane j = column j), pivots are broadcast by shuffles, and the
-// reciprocal square root is an FP32 seed + two FP64 Newton steps: ~200 cycles per pivot, no barrier in the chain.
+// reciprocal square root is an FP32 seed + two FP64 Newton steps: no barrier in the chain.
 __device__ __forceinline__ double shfl_d(double v, int src) { return __shfl_sync(0xffffffffu, v, src); }
 
 // compile-time loop: register arrays must only ever be indexed by constants (a loop the unroller leaves rolled would push

@@ -118,8 +118,8 @@ capital_status_t memops_issue(capital_ctx* ctx, cudaStream_t st, const FlagList&
       ops[i].waitValue.value64 = fl.v[i];
       // FLUSH: "the device is permitted to reorder remote writes internally" (cuda.h, CUstreamWaitValue_flags) -- without it a
       // wait satisfied by a peer's flag does not make that peer's EARLIER stores (partial sums written by its GEMM epilogue over
-      // NVLink) visible to the kernels that follow the wait.  Observed as 1e-10-level, run-to-run varying errors at n = 32768 on
-      // real NVLink (profiles/r02c_coherence_bug_notes.md).
+      // NVLink) visible to the kernels that follow the wait.  Observed as small, run-to-run varying errors of the distributed
+      // factorization over real NVLink.
       ops[i].waitValue.flags = CU_STREAM_WAIT_VALUE_GEQ | (flush ? CU_STREAM_WAIT_VALUE_FLUSH : 0);
     } else {
       ops[i].writeValue.operation = CU_STREAM_MEM_OP_WRITE_VALUE_64;

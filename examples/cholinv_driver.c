@@ -20,7 +20,7 @@ int main(int argc, char** argv) {
   capital_grid_t grid;
   if (capital_grid_square(1, 0, 1, layout, num_chunks, &grid) != CAPITAL_OK) { fprintf(stderr, "bad grid\n"); return 1; }
   capital_ctx* ctx = NULL;
-  if (capital_create(&ctx, &grid, 0, NULL) != CAPITAL_OK) { fprintf(stderr, "capital_create failed: no sm_100 device (there is no CPU fallback)\n"); return 1; }
+  if (capital_create(&ctx, &grid, 0, NULL) != CAPITAL_OK) { fprintf(stderr, "capital_create failed: no sm_90 device (there is no CPU fallback)\n"); return 1; }
   const size_t tri = (size_t)n * (n + 1) / 2;
   double* A = (double*)malloc(sizeof(double) * n * n);
   double* R = (double*)malloc(sizeof(double) * tri);

@@ -1,4 +1,4 @@
-/* capital_b200 -- C ABI of the B200-native CholInv / CholeskyQR2 hot path.
+/* capital_b200 -- C ABI of the H100-native CholInv / CholeskyQR2 hot path.
  *
  * Drop-in boundary for the factorization entry points of tbennun/capital (a header-only C++14
  * template library; it has no FFI of its own, so each entry point below names the reference
@@ -11,7 +11,7 @@
  * Pointers passed to the compute entry points may be device pointers (resident HBM, the fast
  * path) or host pointers (the library stages them through pinned buffers: this is the
  * "reference-facing" call a C++ caller of the reference would make).  There is NO CPU fallback:
- * every entry point fails with CAPITAL_ERR_CUDA when no sm_100 device is usable.
+ * every entry point fails with CAPITAL_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef CAPITAL_B200_H
 #define CAPITAL_B200_H
@@ -31,7 +31,7 @@ typedef struct capital_ctx capital_ctx;
 typedef enum {
   CAPITAL_OK = 0,
   CAPITAL_ERR_INVALID = 1,     /* bad argument (the reference would assert: cholinv.hpp:9,81) */
-  CAPITAL_ERR_CUDA = 2,        /* CUDA runtime / driver failure, or no sm_100 device */
+  CAPITAL_ERR_CUDA = 2,        /* CUDA runtime / driver failure, or no sm_90 device */
   CAPITAL_ERR_NOT_SPD = 3,     /* non-positive pivot in a base case (reference drops LAPACKE info: lapack/interface.hpp:39) */
   CAPITAL_ERR_COMM = 4,        /* NCCL failure */
   CAPITAL_ERR_UNSUPPORTED = 5  /* grid / policy combination outside the hot path */
@@ -121,7 +121,7 @@ capital_status_t capital_profile_end(capital_ctx* ctx, double* kernel_ms, double
  * 6 flag signal, 7 peer DMA, 8 layout kernel), start ms, end ms, three kind-specific numbers (GEMM: m, n, k), 0. */
 capital_status_t capital_timeline_begin(capital_ctx* ctx);
 capital_status_t capital_timeline_end(capital_ctx* ctx, double* out, int64_t cap_records, int64_t* n_records);
-/* FP64 tensor-pipe ceiling of this device right now: a register-resident DMMA.8x8x4 loop on every SM (~50 ms), CUDA-event timed.
+/* FP64 tensor-pipe ceiling of this device right now: a register-resident DMMA.16x8x16 loop on every SM (~15 ms), CUDA-event timed.
  * The denominator of bench.py's roofline fraction. */
 capital_status_t capital_probe_dmma_f64(capital_ctx* ctx, double* tflops, double* ms);
 
@@ -189,7 +189,7 @@ capital_status_t capital_blas_gemm_tn_f64(capital_ctx* ctx, int64_t m, int64_t n
 /* EXPERIMENTAL, OFF BY DEFAULT -- BASELINE config 5 ("FP32/TF32 Cholesky, mixed-precision trailing update with FP64 panel").
  * The reference has no float BLAS path (src/blas/interface.hpp:43-97 is double only): this is an extension of the blas::engine seam,
  * not a replacement of a reference entry point.  capital_blas_gemm_tn_tf32: the product of capital_blas_gemm_tn_f64 (FP64 operands
- * and result, only the CAPITAL_GEMM_C_UPPER flag) computed on the TF32 tensor cores (tcgen05.mma.kind::tf32, accumulator in TMEM);
+ * and result, only the CAPITAL_GEMM_C_UPPER flag) computed on the TF32 tensor cores (wgmma.mma_async .tf32, FP32 accumulators in registers);
  * passes = 1: operands rounded to TF32 (relative error ~ 5e-4 per product), passes = 3: operands split hi + lo (FP32-class).
  * capital_set_trailing_precision(ctx, 0 | 1 | 3): cholinv::factor runs its trailing updates A22 -= R12^T R12 (cholinv.hpp:131-134,
  * summa::syrk) in that mode; base cases, R12, the inverse and every other product stay FP64.  Single GPU and c = 1 grids.

@@ -3,7 +3,7 @@
 Nothing in the product path (capital_b200/, the C-ABI library, bench.py's GPU arm) may import this
 module; it is the checker used by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg.
 
-Each function cites the reference file:line it restates (paths relative to /root/reference).  The
+Each function cites the reference file:line it restates (paths relative to the reference repository's root).  The
 restatement is pinned two ways (tests/test_oracle.py): against the golden dumps produced by the
 reference itself, compiled here by oracle/build_ref.sh (tests/golden/*.npz, made by
 tests/golden/make_golden.py), and against scipy's LAPACK on the same closed-form inputs.

@@ -2,20 +2,18 @@
 
 1. GATING -- BASELINE-size parity of the default FP64 path: n = 16384 factors elementwise against cuSOLVER potrf + a triangular solve.
 
-2. XPASS/XFAIL -- the EXPERIMENTAL mixed-precision path (BASELINE config 5): trailing updates on the TF32 tensor cores (tcgen05 + TMEM,
-   capital_b200/csrc/gemm_tf32.cu), FP64 everywhere else; off by default in the library.  The kernel was written after the round's GPU
-   budget was spent: it assembles for sm_100a (UTCHMMA / LDTM / UTMALDG in the SASS) but the run of THIS file is its first execution.
-   Hence every case runs in a child process with its own CUDA context and a timeout (the kernel's mbarrier waits are bounded too) and
-   is xfail(strict=False): an XPASS in the report means the path computed the right numbers on this device, an XFAIL that it did not;
-   neither touches the FP64 product path.  Gates (no reference float path exists, src/blas/interface.hpp:43-97: the FP64 results are
+2. GATING -- the EXPERIMENTAL mixed-precision path (BASELINE config 5): trailing updates on the TF32 tensor cores (wgmma,
+   capital_b200/csrc/gemm_tf32.cu), FP64 everywhere else; off by default in the library.  Every case runs in a child process with its
+   own CUDA context and a timeout (the kernel's mbarrier waits are bounded too), so that nothing it does can touch the FP64 product
+   path of the parent.  Gates (no reference float path exists, src/blas/interface.hpp:43-97: the FP64 results are
    the yardstick):
      product:       |C - C_fp64| / max(|A|^T |B|) <= 5e-4 (TF32 operands) / 2e-6 (split operands, 3 passes)
      factorization: residual ||A - R^T R||_F / ||A||_F <= 1e-6 (TF32) / 1e-8 (3 x TF32) at n = 4096 (CPU emulation of the rounding,
                     tools/tf32_emulate.py: 5e-9 / 1e-10), and > 1e-13 with the TF32 kernel's launch counter > 0 -- i.e. the
                     tensor-core path really ran.
 
-3. XPASS/XFAIL -- split = 2 of the FP64 path against the reference's dump and the oracle (a parameter added to the parity set after the
-   GPU budget was spent; its schedule is replayed on CPU, its oracle is pinned on CPU)."""
+3. GATING -- split = 2 of the FP64 path against the reference's dump and the oracle (its schedule is replayed on CPU, its oracle is
+   pinned on CPU)."""
 import json
 import os
 import subprocess
@@ -25,7 +23,6 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-WHY = "TF32 tcgen05 path: written without GPU access, this run is its first execution (XPASS = it works)"
 
 
 def worker(*args, timeout=600):
@@ -60,7 +57,6 @@ def test_cholinv_baseline_size_elementwise_against_cusolver(ci):
     torch.cuda.empty_cache()
 
 
-@pytest.mark.xfail(strict=False, reason=WHY)
 def test_tf32_product_against_fp64():
     out = worker("gemm")["gemm"]
     for c in out:
@@ -71,7 +67,6 @@ def test_tf32_product_against_fp64():
     assert any(c["passes"] == 1 and c["rel_err"] > 1e-9 for c in out)
 
 
-@pytest.mark.xfail(strict=False, reason=WHY)
 def test_cholinv_mixed_precision_trailing_update():
     d = worker("cholinv", 4096, -3)
     assert d["tf32_launches"]["f64"] == 0 and d["tf32_launches"]["tf32"] > 0 and d["tf32_launches"]["tf32x3"] > 0
@@ -81,8 +76,7 @@ def test_cholinv_mixed_precision_trailing_update():
     assert d["R_rel_diff"]["tf32"] <= 1e-4 and d["R_rel_diff"]["tf32x3"] <= 1e-6
 
 
-# ---- not TF32: a parameter of the FP64 path whose first GPU run is this file too (kept here so that it cannot stop the suite early) ----
-@pytest.mark.xfail(strict=False, reason="split = 2 was added to the parity set after the round's GPU budget was spent: first GPU run (XPASS = parity holds)")
+# ---- not TF32: split = 2 of the FP64 path ----
 def test_cholinv_uneven_split_matches_reference_dump_and_oracle():
     """split = 2 (cholinv.hpp:92,107: the left child gets a quarter of the node): the reference's own dump, elementwise, and the numpy
     restatement (pinned to that dump on CPU) at a ragged size."""

@@ -1,6 +1,6 @@
 // Probe: does a flag written after a LARGE peer copy ever overtake the tail of the data?  (2 processes, 2 GPUs)
 // rank 0: [memcpy N bytes to rank 1's buffer] [cuStreamWriteValue64 flag on rank 1]   rank 1: [cuStreamWaitValue64] [kernel counts wrong words, tail first]
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o probe_bigcopy probe_bigcopy.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o probe_bigcopy probe_bigcopy.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

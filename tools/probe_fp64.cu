@@ -1,4 +1,4 @@
-// Microbenchmark: FP64 pipe ceilings on sm_100a (DFMA vs DMMA.8x8x4). Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o probe_fp64 probe_fp64.cu
+// Microbenchmark: FP64 pipe ceilings on sm_90a (DFMA vs DMMA.8x8x4). Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o probe_fp64 probe_fp64.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do{cudaError_t e=(x); if(e!=cudaSuccess){printf("CUDA error %s at %d\n",cudaGetErrorString(e),__LINE__); return 1;}}while(0)

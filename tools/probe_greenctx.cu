@@ -1,7 +1,7 @@
 // Probe: green contexts (SM partitions) driven through runtime-API launches.
 // Question: can the deferred ("far") GEMMs be confined to N-8k SMs so that the latency-critical chain kernels (8-CTA cluster,
 // 146 KB smem per CTA) always find free SMs instead of waiting ~1 ms for a 128x128 tile to retire?
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o probe_greenctx probe_greenctx.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o probe_greenctx probe_greenctx.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>
@@ -102,7 +102,7 @@ int main() {
       CK(cudaStreamCreateWithPriority(&lowp, cudaStreamNonBlocking, lo));
       cudaStream_t fs = mode == 1 ? far : lowp;
       const long long far_cycles = 4000000;  // ~2 ms per CTA
-      if (mode) spin_kernel<<<148 * 4, 128, smem, fs>>>(far_cycles, nullptr);
+      if (mode) spin_kernel<<<132 * 4, 128, smem, fs>>>(far_cycles, nullptr);
       // give the far kernel time to occupy the machine
       spin_kernel<<<1, 32, 1024, chain>>>(400000, nullptr);
       CK(cudaEventRecord(e0, chain));

@@ -3,7 +3,7 @@
 // NP processes (fork before CUDA init), rank r on GPU r % ndev (or all on GPU 0 with same_device=1).
 // Measures: IPC mapping, DMA push bandwidth (contiguous / strided 2D), SM remote-store and remote-load bandwidth,
 // flag ping-pong latency with signal/wait kernels and with stream memory ops (cuStreamWriteValue64 / WaitValue64).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o probe_p2p probe_p2p.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o probe_p2p probe_p2p.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -115,7 +115,7 @@ int main(int argc, char** argv) {
   // ---- D: SM remote stores / loads (rank 0 -> 1) ----
   host_barrier(sh, np, 4);
   if (rank == 0) {
-    for (int blocks : {16, 148, 592}) {
+    for (int blocks : {16, 132, 528}) {
       store16_kernel<<<blocks, 256, 0, st>>>((double2*)pdata[peer], BYTES / 16, 1.0);
       CK(cudaEventRecord(e0, st));
       for (int i = 0; i < 3; i++) store16_kernel<<<blocks, 256, 0, st>>>((double2*)pdata[peer], BYTES / 16, 1.0);
@@ -124,15 +124,15 @@ int main(int argc, char** argv) {
     }
     {
       CK(cudaEventRecord(e0, st));
-      for (int i = 0; i < 3; i++) store_epi_kernel<<<148, 256, 0, st>>>(pdata[peer], 4096, 4096, 4096, 2.0);
+      for (int i = 0; i < 3; i++) store_epi_kernel<<<132, 256, 0, st>>>(pdata[peer], 4096, 4096, 4096, 2.0);
       CK(cudaEventRecord(e1, st)); CK(cudaEventSynchronize(e1)); CK(cudaEventElapsedTime(&ms, e0, e1));
       printf("D SM remote store, epilogue pattern (8B, 64B runs) 4096x4096: %.1f GB/s\n", 3 * 4096.0 * 4096 * 8 / ms / 1e6);
       CK(cudaEventRecord(e0, st));
-      for (int i = 0; i < 3; i++) store_epi_kernel<<<148, 256, 0, st>>>(data, 4096, 4096, 4096, 2.0);
+      for (int i = 0; i < 3; i++) store_epi_kernel<<<132, 256, 0, st>>>(data, 4096, 4096, 4096, 2.0);
       CK(cudaEventRecord(e1, st)); CK(cudaEventSynchronize(e1)); CK(cudaEventElapsedTime(&ms, e0, e1));
       printf("D SM LOCAL store, epilogue pattern 4096x4096: %.1f GB/s\n", 3 * 4096.0 * 4096 * 8 / ms / 1e6);
     }
-    for (int blocks : {148, 592}) {
+    for (int blocks : {132, 528}) {
       CK(cudaEventRecord(e0, st));
       for (int i = 0; i < 3; i++) load16_kernel<<<blocks, 256, 0, st>>>((const double2*)pdata[peer], BYTES / 16, d_out);
       CK(cudaEventRecord(e1, st)); CK(cudaEventSynchronize(e1)); CK(cudaEventElapsedTime(&ms, e0, e1));

@@ -1,5 +1,5 @@
 """Child process of tests/test_gpu_zz_late.py (and of bench.py's optional `tf32` record): runs the EXPERIMENTAL TF32 tensor-core path in
-its own CUDA context, so that a fault in it (it was written without a GPU at hand) cannot poison the parent's context, and prints ONE
+its own CUDA context, so that a fault in it cannot poison the parent's context, and prints ONE
 JSON line.  usage: tf32_worker.py gemm | cholinv n bcm | bench n bcm steps"""
 import json
 import os
