@@ -112,7 +112,6 @@ struct HostIO {
   int64_t cols_out = 0, rinv_cols_out = 0;
   bool rinv_streams = false;  // Rinv columns right of the top split are final as soon as R's are (complete_inv == 0)
   cudaEvent_t e_out = nullptr;
-  double *zR = nullptr, *zRinv = nullptr;  // experimental block-wise output: device aliases of the pinned host arrays
 };
 capital_status_t io_event(capital_ctx* ctx, cudaEvent_t* e) {
   if (ctx->io_used == ctx->io_pool.size()) {
@@ -203,27 +202,6 @@ capital_status_t hostio_right_done(void* user, cudaStream_t st) {
   return CAPITAL_OK;
 }
 capital_status_t hostio_inv_cols(void* user, cudaStream_t st, int64_t col_end) { return hostio_emit((HostIO*)user, st, false, col_end); }
-// experimental block-wise output: the block is stored straight from the rect work buffer into its slots of the pinned packed array
-capital_status_t hostio_block_done(void* user, cudaStream_t st, int which, int64_t r0, int64_t r1, int64_t c0, int64_t c1) {
-  HostIO* io = (HostIO*)user;
-  capital_ctx* ctx = io->ctx;
-  cudaEvent_t e;
-  CAP_TRY(io_event(ctx, &e));
-  CAP_CUDA(cudaEventRecord(e, st));
-  CAP_CUDA(cudaStreamWaitEvent(ctx->zc_out, e, 0));
-  CAP_TRY(emit_block_packed(ctx, ctx->zc_out, which ? io->Ri : io->Rm, io->ld, which ? io->zRinv : io->zR, r0, r1, c0, c1, ctx->zc_ctas));
-  for (int64_t c = c0; c < c1; c++) {  // bytes that cross the link: the block clipped to the upper triangle
-    const int64_t re = r1 < c + 1 ? r1 : c + 1;
-    if (re > r0) ctx->counters.d2h_bytes += (re - r0) * 8;
-  }
-  return CAPITAL_OK;
-}
-// device-visible alias of a pinned (cudaHostAlloc / cudaHostRegister) host pointer, or nullptr
-double* host_alias(const void* p) {
-  cudaPointerAttributes at;
-  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-  return at.type == cudaMemoryTypeHost ? (double*)at.devicePointer : nullptr;
-}
 }  // namespace
 
 extern "C" {
@@ -305,8 +283,6 @@ static bool make_green_side_stream(capital_ctx* ctx, int reserve, int prio) {
   ctx->side_deep[0] = (cudaStream_t)gd[0];
   ctx->side_deep[1] = (cudaStream_t)gd[1];
   ctx->green = (void*)g;
-  ctx->side_sms = 0;
-  for (auto& r : far) ctx->side_sms += (int)r.sm.smCount;
   return true;
 }
 
@@ -342,7 +318,6 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   ok = ok && cudaStreamCreateWithFlags(&ctx->copy_out, cudaStreamNonBlocking) == cudaSuccess;
   ok = ok && cudaEventCreate(&ctx->ev_start) == cudaSuccess && cudaEventCreate(&ctx->ev_stop) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaMalloc(&ctx->d_info, sizeof(int)) == cudaSuccess && cudaMalloc(&ctx->d_scalars, 16 * sizeof(double)) == cudaSuccess;
   ok = ok && cudaMemset(ctx->d_info, 0, sizeof(int)) == cudaSuccess;
   cudaDriverEntryPointQueryResult qres;
@@ -352,13 +327,8 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   ctx->encode = (cuTensorMapEncodeTiled_fn)fn;
   if (gemm_tn_init(ctx) != CAPITAL_OK || leaf_init(ctx) != CAPITAL_OK) { capital_destroy(ctx); return CAPITAL_ERR_CUDA; }
   if (const char* e = getenv("CAPITAL_TF32_MIN_K")) ctx->tf32_min_k = atoll(e);
-  if (const char* e = getenv("CAPITAL_KCHUNK")) ctx->kchunk = atoll(e);
   if (const char* e = getenv("CAPITAL_FAR_MIN")) ctx->far_min = atoll(e);
   if (const char* e = getenv("CAPITAL_SIDE_MIN")) ctx->side_min = atoll(e);
-  if (const char* e = getenv("CAPITAL_ZC_OUT")) ctx->zc_mode = atoi(e);
-  if (const char* e = getenv("CAPITAL_ZC_CTAS")) ctx->zc_ctas = atoi(e);
-  if (const char* e = getenv("CAPITAL_ZC_DEPTH")) ctx->zc_depth = atoi(e);
-  if (ctx->zc_mode && cudaStreamCreateWithPriority(&ctx->zc_out, cudaStreamNonBlocking, prio_hi) != cudaSuccess) { capital_destroy(ctx); return CAPITAL_ERR_CUDA; }
   *out = ctx;
   return CAPITAL_OK;
 }
@@ -371,11 +341,9 @@ void capital_destroy(capital_ctx* ctx) {
   for (auto& kv : ctx->pool) if (kv.second.p) cudaFree(kv.second.p);
   if (ctx->d_info) cudaFree(ctx->d_info);
   if (ctx->d_scalars) cudaFree(ctx->d_scalars);
-  if (ctx->pinned) cudaFreeHost(ctx->pinned);
   if (ctx->ev_start) cudaEventDestroy(ctx->ev_start);
   if (ctx->ev_stop) cudaEventDestroy(ctx->ev_stop);
   if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-  if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
   for (cudaEvent_t e : ctx->prof_pool) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->tl_pool) cudaEventDestroy(e);
   if (ctx->side) cudaStreamDestroy(ctx->side);
@@ -389,7 +357,6 @@ void capital_destroy(capital_ctx* ctx) {
   if (ctx->hi) cudaStreamDestroy(ctx->hi);
   if (ctx->copy_in) cudaStreamDestroy(ctx->copy_in);
   if (ctx->copy_out) cudaStreamDestroy(ctx->copy_out);
-  if (ctx->zc_out) cudaStreamDestroy(ctx->zc_out);
   for (cudaEvent_t e : ctx->dep_pool) cudaEventDestroy(e);
   for (cudaEvent_t e : ctx->io_pool) cudaEventDestroy(e);
   if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -431,7 +398,6 @@ capital_status_t capital_release_workspace(capital_ctx* ctx) {
   CAP_TRY(dist_release_peer_maps(ctx));
   for (auto& kv : ctx->pool) if (kv.second.p) CAP_CUDA(cudaFree(kv.second.p));
   ctx->pool.clear();
-  if (ctx->pinned) { CAP_CUDA(cudaFreeHost(ctx->pinned)); ctx->pinned = nullptr; ctx->pinned_bytes = 0; }
   return CAPITAL_OK;
 }
 capital_status_t capital_last_factor_ms(const capital_ctx* ctx_, float* ms) {
@@ -551,17 +517,8 @@ capital_status_t capital_cholinv_factor_f64(capital_ctx* ctx, const double* A_lo
   CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Rm));
   CAP_TRY(ctx->workspace("Ri", (size_t)ld * L * 8, (void**)&Ri));
   CAP_TRY(ctx->workspace("RiT", (size_t)ld * L * 8, (void**)&RiT));
-  // experimental block-wise output: both outputs pinned host arrays, packed, large enough to matter
-  double *zR = nullptr, *zRinv = nullptr;
-  if (ctx->zc_mode && ctx->zc_out && ostruct == CAPITAL_UPPERTRI_PACKED && L >= 2048 && !cap_is_device_ptr(R_local) && !cap_is_device_ptr(Rinv_local)) {
-    zR = host_alias(R_local); zRinv = host_alias(Rinv_local);
-    if (!zR || !zRinv) zR = zRinv = nullptr;
-  }
-  if (zR) { dR = dRinv = nullptr; }
-  else {
-    CAP_TRY(cap_stage_out_begin(ctx, R_local, out_count, "R_out", &dR));
-    CAP_TRY(cap_stage_out_begin(ctx, Rinv_local, out_count, "Rinv_out", &dRinv));
-  }
+  CAP_TRY(cap_stage_out_begin(ctx, R_local, out_count, "R_out", &dR));
+  CAP_TRY(cap_stage_out_begin(ctx, Rinv_local, out_count, "Rinv_out", &dRinv));
   CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
   if (ostruct == CAPITAL_RECT) {
@@ -608,21 +565,14 @@ capital_status_t capital_cholinv_factor_f64(capital_ctx* ctx, const double* A_lo
   } else {
     CAP_TRY(copy_block(ctx, st, L, L, A_local, L, W, ld));  // serialize(A -> R), cholinv.hpp:13
   }
-  io.zR = zR; io.zRinv = zRinv;
-  if (zR) hooks.block_done = hostio_block_done;
-  else if (io.packed && L >= 2048) hooks.left_done = hostio_left_done;  // finished column ranges are packed (and copied out) early
+  if (io.packed && L >= 2048) hooks.left_done = hostio_left_done;  // finished column ranges are packed (and copied out) early
   if (hooks.need_cols) hooks.cols_waited = hostio_cols_waited;
   if (hooks.left_done && (io.hR || io.hRinv)) {  // host outputs: the tail of R and the top-level inverse block stream out too
     hooks.right_done = hostio_right_done;
     if (io.hRinv) hooks.inv_cols = hostio_inv_cols;
   }
   CAP_TRY(cholinv_local(ctx, st, L, W, ld, Rm, ld, Ri, ld, RiT, ld, args->complete_inv != 0, bc, (int)args->split, &hooks));
-  if (zR) {  // every block has been handed to the output stream inside the recursion
-    cudaEvent_t e;
-    CAP_TRY(io_event(ctx, &e));
-    CAP_CUDA(cudaEventRecord(e, ctx->zc_out));
-    CAP_CUDA(cudaStreamWaitEvent(st, e, 0));
-  } else if (ostruct == CAPITAL_UPPERTRI_PACKED) {
+  if (ostruct == CAPITAL_UPPERTRI_PACKED) {
     {  // columns [0, c0) are already packed (and on their way to the host)
       const int64_t c0 = io.cols_out;
       const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = out_count - off;

@@ -39,7 +39,6 @@ struct Rec {
   const CholinvHooks* hooks;
   int64_t far_min;  // trailing updates smaller than this are not split
   int64_t total;      // size of the top-level block
-  int64_t kchunk;     // k extent of one launch of deferred work (bounds how long a deferred tile holds an SM)
   bool base_aligned;  // all four buffers 16-byte aligned with even leading dimensions (cluster kernel uses 16-byte accesses)
 };
 
@@ -74,16 +73,11 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   double* RiT = r.RiT + o * r.ldrit + o;
   const int64_t ldw = r.ldw, ldr = r.ldr, ldri = r.ldri, ldrit = r.ldrit;
   const int64_t s1 = choose_split(r, o, n, complete);
-  const bool blocks = r.hooks && r.hooks->block_done;  // experimental block-wise output (common.cuh)
   if (s1 == 0) {
     if (r.hooks && r.hooks->need_cols) CAP_TRY(r.hooks->need_cols(r.hooks->user, r.M, o + n));
     if (pending) CAP_CUDA(cudaStreamWaitEvent(r.M, pending, 0));
     if (n <= LEAF_MAX) CAP_TRY(leaf_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
     else CAP_TRY(basecase_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
-    if (blocks && depth <= ctx->zc_depth) {  // a leaf above the emission depth: its triangle is a unit of the tiling
-      CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 0, o, o + n, o, o + n));
-      CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 1, o, o + n, o, o + n));
-    }
     return CAPITAL_OK;
   }
   const int64_t s2 = n - s1;
@@ -95,8 +89,6 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   double* Ri22 = Ri + s1 * ldri + s1;
   double* RiT21 = RiT + s1;
 
-  // the skipped inverse block (complete_inv == 0) is part of the output all the same: zeros, written by the caller before the recursion
-  if (blocks && depth < ctx->zc_depth && !complete) CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 1, o, o + s1, o + s1, o + n));
   CAP_TRY(rec(r, o, s1, true, nullptr, depth + 1));
   // right spine only (o + n == total size): everything left of column o + s1 is final for R
   if (depth <= 3 && o + n == r.total && r.hooks && r.hooks->left_done) CAP_TRY(r.hooks->left_done(r.hooks->user, r.M, o + s1, depth));
@@ -117,7 +109,6 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
     if (pending) CAP_CUDA(cudaStreamWaitEvent(r.M, pending, 0));  // the parent's deferred update covers W12 and W22
     CAP_TRY(gemm_tn(ctx, r.M, s1, s2, s1, 1.0, Ri, ldri, W12, ldw, 0.0, R12, ldr, CAPITAL_GEMM_A_UPPER));
   }
-  if (blocks && depth < ctx->zc_depth) CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 0, o, o + s1, o + s1, o + n));  // R12 is final
   cudaEvent_t e_r12 = nullptr, e_tt = nullptr, e_far = nullptr;
   const bool use_side = r.S != nullptr && s1 >= r.ctx->side_min;
   if (use_side) {
@@ -139,9 +130,9 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
                            CAPITAL_GEMM_C_UPPER, tf));
     } else {
       CAP_TRY(gemm_tn(ctx, r.M, h, h, s1, -1.0, R12, ldr, R12, ldr, 1.0, W22, ldw, CAPITAL_GEMM_C_UPPER));
-      CAP_TRY(gemm_tn_chunked(ctx, r.S, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0, r.kchunk));
-      CAP_TRY(gemm_tn_chunked(ctx, r.S, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
-                              CAPITAL_GEMM_C_UPPER, r.kchunk));
+      CAP_TRY(gemm_tn(ctx, r.S, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0));
+      CAP_TRY(gemm_tn(ctx, r.S, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
+                      CAPITAL_GEMM_C_UPPER));
     }
     CAP_TRY(new_event(ctx, &e_far));
     CAP_CUDA(cudaEventRecord(e_far, r.S));
@@ -153,7 +144,7 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   if (complete) {
     // inverse combine, first half (cholinv.hpp:151): T^T = R12^T Rinv11^T  (B = RiT11, lower triangular) -- nobody needs
     // it before the right child is done, so it goes to the deferred stream.
-    CAP_TRY(gemm_tn_chunked(ctx, tS, s2, s1, s1, 1.0, R12, ldr, RiT, ldrit, 0.0, W21, ldw, CAPITAL_GEMM_B_LOWER, use_side ? r.kchunk : 0));
+    CAP_TRY(gemm_tn(ctx, tS, s2, s1, s1, 1.0, R12, ldr, RiT, ldrit, 0.0, W21, ldw, CAPITAL_GEMM_B_LOWER));
     if (use_side) {
       CAP_TRY(new_event(ctx, &e_tt));
       CAP_CUDA(cudaEventRecord(e_tt, r.S));
@@ -176,18 +167,13 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
         const int64_t c0 = edge[i], c1 = edge[i + 1];
         if (c1 <= c0) continue;
         CAP_TRY(gemm_tn_off(ctx, r.M, s1, c1 - c0, c1, -1.0, W21, ldw, Ri22 + c0 * ldri, ldri, 0.0, Ri12 + c0 * ldri, ldri,
-                            CAPITAL_GEMM_B_UPPER, 0, (int)c0));
+                            CAPITAL_GEMM_B_UPPER, (int)c0));
         CAP_TRY(r.hooks->inv_cols(r.hooks->user, r.M, o + s1 + c1));
       }
     } else {
       CAP_TRY(gemm_tn(ctx, r.M, s1, s2, s2, -1.0, W21, ldw, Ri22, ldri, 0.0, Ri12, ldri, CAPITAL_GEMM_B_UPPER));
     }
-    if (blocks && depth < ctx->zc_depth) CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 1, o, o + s1, o + s1, o + n));
     CAP_TRY(transpose_block(ctx, r.M, s1, s2, Ri12, ldri, RiT21, ldrit, 1.0));
-  }
-  if (blocks && depth == ctx->zc_depth) {  // diagonal triangle of a node at the emission depth
-    CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 0, o, o + n, o, o + n));
-    CAP_TRY(r.hooks->block_done(r.hooks->user, r.M, 1, o, o + n, o, o + n));
   }
   return CAPITAL_OK;
 }
@@ -209,7 +195,7 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
     if (S) CAP_CUDA(cudaStreamWaitEvent(S, e_in, 0));
   }
   const bool aligned = ((((uintptr_t)W | (uintptr_t)R | (uintptr_t)Ri | (uintptr_t)RiT) & 15) == 0) && !((ldw | ldr | ldri | ldrit) & 1);
-  Rec r{ctx, M, S, W, R, Ri, RiT, ldw, ldr, ldri, ldrit, bc, split, hooks, ctx->far_min, n, ctx->kchunk, aligned};
+  Rec r{ctx, M, S, W, R, Ri, RiT, ldw, ldr, ldri, ldrit, bc, split, hooks, ctx->far_min, n, aligned};
   // a top-level node the reference treats as its base case (n <= bc, cholinv.hpp:93-104) gets the FULL inverse whatever complete_inv
   // says; the skip of cholinv.hpp:147 only exists where the top node really splits at n >> split
   if (!cholinv_node_splits(n, bc, split)) complete_top = true;

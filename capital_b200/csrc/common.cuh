@@ -43,29 +43,21 @@ struct capital_ctx {
   cudaStream_t stream = nullptr;   // main stream (caller's or owned)
   cudaStream_t side = nullptr;     // low-priority stream: deferred ("far") trailing updates, T^T products; lives in a green context
   void* green = nullptr;           // (CUgreenCtx) SM partition of the deferred stream, see make_green_side_stream (api.cu)
-  int side_sms = 0;                // SMs of that partition (0: no partition)
   cudaStream_t side_deep[2] = {nullptr, nullptr};  // deferred streams of recursion depths 1 and 2 (multi-GPU schedule), same partition, rising priority
   cudaStream_t hi = nullptr;       // high-priority stream: the critical chain of the recursion
   cudaStream_t copy_in = nullptr, copy_out = nullptr;  // H2D / D2H streams of the host-pointer path
-  // EXPERIMENTAL, off by default [env CAPITAL_ZC_OUT=1]: host outputs leave block by block through a kernel that stores straight
-  // into the pinned packed arrays (partial columns can leave as soon as they are final)
-  cudaStream_t zc_out = nullptr;
-  int zc_mode = 0, zc_ctas = 8, zc_depth = 3;  // [env CAPITAL_ZC_CTAS, CAPITAL_ZC_DEPTH]
   std::vector<cudaEvent_t> dep_pool;  // dependency events (timing disabled), recycled per factor call
   size_t dep_used = 0;
   std::vector<cudaEvent_t> io_pool;   // events of the host-pointer streaming path
   size_t io_used = 0;
   bool own_stream = false;
-  cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_fork = nullptr, ev_join = nullptr;
+  cudaEvent_t ev_start = nullptr, ev_stop = nullptr, ev_fork = nullptr;
   cuTensorMapEncodeTiled_fn encode = nullptr;
   capital_counters_t counters{};
   std::string err;
   int* d_info = nullptr;           // device flag: first non-SPD pivot (0 = ok)
   double* d_scalars = nullptr;     // device scratch for reductions (16 doubles)
   std::map<std::string, DeviceBuf> pool;  // named, grow-only workspace (the reference's `info` tables, cholinv.h:35-40)
-  // pinned staging for host-pointer callers
-  void* pinned = nullptr;
-  size_t pinned_bytes = 0;
   // multi-GPU: peer layer (peer.cuh) -- IPC-mapped arenas and flags; NCCL (dlopen'ed) only bootstraps the handle exchange
   void* comm_world = nullptr;          // ncclComm_t, when capital_comm_init was used
   void* peer = nullptr;                // Peer*
@@ -76,7 +68,6 @@ struct capital_ctx {
   // per-launch timing of the dominant kernel (gemm_tn 128x128), off by default
   struct ProfRec { cudaEvent_t e0, e1; double flops; };
   bool profiling = false;
-  int64_t kchunk = 0;       // k-chunking of deferred GEMMs (env CAPITAL_KCHUNK); 0 = off
   int64_t far_min = 2048;   // trailing updates at least this large are split into near (critical) / far (deferred)   [env CAPITAL_FAR_MIN]
   int64_t side_min = 1024;  // nodes whose left part is at least this large defer T^T to the low-priority stream      [env CAPITAL_SIDE_MIN]
   bool no_overlap = false;  // debug / measurement: run the recursion on one stream
@@ -112,7 +103,6 @@ struct capital_ctx {
 
   void set_error(const std::string& s) { err = s; }
   capital_status_t workspace(const std::string& name, size_t bytes, void** out);
-  capital_status_t pinned_buf(size_t bytes, void** out);
 };
 
 // ---- gemm_tn.cu -------------------------------------------------------------------------------
@@ -143,14 +133,12 @@ struct GemmOperands {
   int64_t lda = 0, ldb = 0;
 };
 capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmOperands& ops,
-                           double beta, double* C, int64_t ldc, int flags, int koff, int noff, const GemmXDev* x);
+                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x);
 capital_status_t gemm_tn(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                          int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags);
 
 capital_status_t gemm_tn_off(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int koff, int noff = 0);
-capital_status_t gemm_tn_chunked(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                                 int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int64_t kc);
+                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff);
 capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags);
 capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
@@ -174,8 +162,6 @@ capital_status_t zero_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, int
 capital_status_t zero_band(capital_ctx* ctx, cudaStream_t st, int64_t n, double* a, int64_t ld);
 capital_status_t pack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* packed,
                             int zero_diag, int64_t col_begin = 0, int64_t col_end = -1);
-capital_status_t emit_block_packed(capital_ctx* ctx, cudaStream_t st, const double* src, int64_t lds, double* packed, int64_t r0, int64_t r1,
-                                   int64_t c0, int64_t c1, int ctas);
 capital_status_t unpack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* packed, double* dst, int64_t ldd);
 capital_status_t triu_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst,
                            int64_t ldd, int zero_diag);
@@ -201,8 +187,7 @@ capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const d
 // local (single-GPU) recursive CholInv on dense n x n blocks; W is destroyed (Schur complements).
 // Optional callbacks of the top-level call (host-pointer path): `need_cols` makes `st` wait until columns [0, col_end)
 // of W have arrived from the host; `left_done` fires after each left child on the right spine (depth <= 3), when columns
-// [0, col_end) of R are final
-// and Rinv are final.
+// [0, col_end) of R are final, and those of Rinv too at depth 0.
 struct CholinvHooks {
   void* user;
   capital_status_t (*need_cols)(void* user, cudaStream_t st, int64_t col_end);
@@ -214,10 +199,6 @@ struct CholinvHooks {
   int64_t (*cols_waited)(void* user);
   capital_status_t (*right_done)(void* user, cudaStream_t st);
   capital_status_t (*inv_cols)(void* user, cudaStream_t st, int64_t col_end);
-  // optional, exclusive with left_done / right_done / inv_cols: rows [r0, r1) x columns [c0, c1) (clipped to the upper triangle) of
-  // R (which = 0) or Rinv (which = 1) are final on stream `st`.  Fired for the off-diagonal block of every node above depth
-  // ctx->zc_depth and for the diagonal triangle of the nodes at that depth (or leaves above it): together they tile the triangle.
-  capital_status_t (*block_done)(void* user, cudaStream_t st, int which, int64_t r0, int64_t r1, int64_t c0, int64_t c1);
 };
 // allow_side = false keeps everything on `st` (the distributed base case runs on the critical chain and must not queue behind
 // the deferred stream's GEMMs).

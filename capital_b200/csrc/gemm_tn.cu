@@ -27,7 +27,6 @@ struct GemmParams {
   int rowoffA, rowoffB;  // element offset of the operand's first row inside its (16B-aligned) tensor map
   int flags;
   int noff;    // column index of this window of B / C inside the full operand (column-chunked launches)
-  int koff;    // row index of this window inside the full operand (k-chunked launches keep the triangular k ranges right)
   int ksplit;  // gridDim.z chunks of the k range; > 1 => epilogue accumulates with atomics (C pre-initialised, beta ignored)
   int ncls;    // operand classes: the contraction runs over ncls (A_i, B_i) pairs with identical shapes (SUMMA k-slices, summa.hpp:185-193)
   int gm, gn;  // tile grid
@@ -121,13 +120,13 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
   if ((flags & CAPITAL_GEMM_C_UPPER) && m0 > n0g + BN - 1) return;  // tile strictly below the diagonal
 
   int kb = 0, ke = p.K;
-  if (flags & CAPITAL_GEMM_A_UPPER) ke = min(ke, m0 + BM - p.koff);
-  if (flags & CAPITAL_GEMM_A_LOWER) kb = max(kb, m0 - p.koff);
-  if (flags & CAPITAL_GEMM_B_UPPER) ke = min(ke, n0g + BN - p.koff);
-  if (flags & CAPITAL_GEMM_B_LOWER) kb = max(kb, n0g - p.koff);
+  if (flags & CAPITAL_GEMM_A_UPPER) ke = min(ke, m0 + BM);
+  if (flags & CAPITAL_GEMM_A_LOWER) kb = max(kb, m0);
+  if (flags & CAPITAL_GEMM_B_UPPER) ke = min(ke, n0g + BN);
+  if (flags & CAPITAL_GEMM_B_LOWER) kb = max(kb, n0g);
   kb &= ~(BK - 1);
   int nk = ke > kb ? (ke - kb + BK - 1) / BK : 0;
-  if (nk == 0 && p.beta == 1.0 && p.ksplit <= 1) return;  // nothing to add (k-chunk entirely outside the operand's triangle); same on every layer
+  if (nk == 0 && p.beta == 1.0 && p.ksplit <= 1) return;  // nothing to add (the tile's k range lies outside the operand's triangle); same on every layer
   if (p.ksplit > 1) {  // this CTA's contiguous chunk of k tiles
     const int per = (nk + p.ksplit - 1) / p.ksplit;
     const int t0 = min(nk, (int)blockIdx.z * per), t1 = min(nk, t0 + per);
@@ -297,11 +296,11 @@ struct GemmExtra {
 };
 template <class Cfg>
 capital_status_t launch(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, GemmOperands ops, double beta, double* C,
-                        int64_t ldc, int flags, int ksplit, int koff, int noff, const GemmXDev* x, const GemmExtra* ex = nullptr) {
+                        int64_t ldc, int flags, int ksplit, int noff, const GemmXDev* x, const GemmExtra* ex = nullptr) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN;
   GemmParams p{};
   if (ex) { p.Ct = ex->Ct; p.ldct = ex->ldct; p.no_c = ex->no_c; p.kpart = ex->kpart; p.kstride = ex->kstride; p.ldk = ex->ldk; }
-  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc; p.ksplit = ksplit; p.koff = koff; p.noff = noff;
+  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc; p.ksplit = ksplit; p.noff = noff;
   p.ncls = ops.ncls;
   // TMA fetches 16-byte granules: a window that starts on an odd row (8-byte aligned only) cannot be addressed by
   // box coordinates, so it is first copied to an aligned scratch (O(k m) bytes against O(k m n) flops; only odd
@@ -441,15 +440,15 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
   ops.A[0] = A; ops.B[0] = B; ops.lda = lda; ops.ldb = ldb;
   if (ks == 1) {  // one chunk: the tile is stored straight into C
     ctx->counters.kernel_launches--;
-    if (big) return launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, 0, nullptr);
-    return launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, 0, nullptr);
+    if (big) return launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, nullptr);
+    return launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, nullptr);
   }
   GemmExtra ex;
   ex.ldk = round_up(m, 2); ex.kstride = ex.ldk * n;
   CAP_TRY(ctx->workspace("splitk_part", (size_t)ks * ex.kstride * 8, (void**)&ex.kpart));
   const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
-  if (big) CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, 0, nullptr, &ex)));
-  else CAP_TRY((launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, 0, nullptr, &ex)));
+  if (big) CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, nullptr, &ex)));
+  else CAP_TRY((launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, nullptr, &ex)));
   ctx->tl_end(st, tli);
   const long long total = m * n;
   const int gr = (int)std::min<long long>((total + 255) / 256, (long long)ctx->num_sms * 4);
@@ -476,42 +475,28 @@ capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
   const bool big = gemm_uses_big(ctx, m, n);
   const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
   capital_status_t rs;
-  if (big) rs = launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, 0, nullptr, &ex);
-  else rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, 0, nullptr, &ex);
+  if (big) rs = launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, nullptr, &ex);
+  else rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, nullptr, &ex);
   ctx->tl_end(st, tli);
   return rs;
 }
 
-// Same product issued as a sequence of k-chunked launches (C accumulates).  Used for deferred work on the low-priority
-// stream: a 128x128 tile with k = 8192 occupies its SM for ~1 ms, which would make the latency-critical kernels of the
-// high-priority stream wait that long for an SM; chunks of `kc` bound the wait to kc/16 k-tiles.
-capital_status_t gemm_tn_chunked(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                                 int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int64_t kc) {
-  if (kc <= 0 || k <= kc + kc / 2) return gemm_tn(ctx, st, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags);
-  for (int64_t k0 = 0; k0 < k; k0 += kc) {
-    const int64_t kk = (k - k0 < kc + kc / 2) ? k - k0 : kc;
-    CAP_TRY(gemm_tn_off(ctx, st, m, n, kk, alpha, A + k0, lda, B + k0, ldb, k0 == 0 ? beta : 1.0, C, ldc, flags, (int)k0, 0));
-    if (kk != kc) break;
-  }
-  return CAPITAL_OK;
-}
-
 capital_status_t gemm_tn(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                          int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags) {
-  return gemm_tn_off(ctx, st, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags, 0, 0);
+  return gemm_tn_off(ctx, st, m, n, k, alpha, A, lda, B, ldb, beta, C, ldc, flags, 0);
 }
 
 capital_status_t gemm_tn_off(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int koff, int noff) {
+                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff) {
   GemmOperands ops;
   ops.A[0] = A; ops.B[0] = B; ops.lda = lda; ops.ldb = ldb;
-  return gemm_tn_x(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, koff, noff, nullptr);
+  return gemm_tn_x(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, noff, nullptr);
 }
 
 // General form: `ops.ncls` operand classes, optional fused depth exchange (see GemmXDev).  With an exchange every layer must call
 // this with the same shapes and flags (the tile grid and the tile ownership are functions of them only).
 capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmOperands& ops,
-                           double beta, double* C, int64_t ldc, int flags, int koff, int noff, const GemmXDev* x) {
+                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x) {
   if (m <= 0 || n <= 0) return CAPITAL_OK;
   bool bad = k < 0 || ops.lda < k || ops.ldb < k || ldc < m || (ops.lda & 1) || (ops.ldb & 1) || ops.ncls < 1 || ops.ncls > GEMM_NCLS_MAX;
   for (int c = 0; !bad && c < ops.ncls; c++) bad = !ops.A[c] || !ops.B[c] || ((uintptr_t)ops.A[c] & 7) || ((uintptr_t)ops.B[c] & 7);
@@ -530,7 +515,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
   const bool atri = flags & (CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_A_LOWER), btri = flags & (CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_B_LOWER);
   if (atri && btri) f = 2.0 * (double)m * (double)n * (double)k / 3.0;
   else if (atri) f = (double)n * (double)m * (double)(m + 1);
-  else if (btri && (flags & CAPITAL_GEMM_B_UPPER) && noff > 0 && koff == 0 && k >= noff + n) f = (double)m * (double)n * (double)(2 * (int64_t)noff + n + 1);
+  else if (btri && (flags & CAPITAL_GEMM_B_UPPER) && noff > 0 && k >= noff + n) f = (double)m * (double)n * (double)(2 * (int64_t)noff + n + 1);
   else if (btri) f = (double)m * (double)n * (double)(n + 1);
   else if (flags & CAPITAL_GEMM_C_UPPER) f = (double)k * (double)m * (double)(m + 1);
   f *= ops.ncls;
@@ -544,7 +529,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
       CAP_CUDA(cudaEventRecord(e0, st));
     }
     const int tli = ctx->tl_begin(st, 1, (double)m, (double)n, (double)k * ops.ncls);
-    CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, koff, noff, x)));
+    CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, x)));
     ctx->tl_end(st, tli);
     if (ctx->profiling) {
       CAP_CUDA(cudaEventRecord(e1, st));
@@ -553,7 +538,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
     return CAPITAL_OK;
   }
   const int tli = ctx->tl_begin(st, 2, (double)m, (double)n, (double)k * ops.ncls);
-  const capital_status_t rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, koff, noff, x);
+  const capital_status_t rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, x);
   ctx->tl_end(st, tli);
   return rs;
 }

@@ -52,18 +52,6 @@ __global__ void pack_upper_kernel(long long c0, long long n, const double* src, 
     for (long long j = threadIdx.x; j <= i; j += blockDim.x) d[j] = (zero_diag && j == i) ? 0.0 : s[j];
   }
 }
-// rows [r0, min(r1, col + 1)) of columns [c0, c1) of a rect matrix -> their slots of the packed upper triangle.  `packed` may be
-// the device alias of a pinned host array: each column is one contiguous run of coalesced 8-byte stores, a handful of CTAs
-// keeps the PCIe link busy.
-__global__ void emit_block_packed_kernel(const double* src, long long lds, double* packed, long long r0, long long r1,
-                                         long long c0, long long c1) {
-  for (long long i = c0 + blockIdx.x; i < c1; i += gridDim.x) {
-    const double* s = src + i * lds;
-    double* d = packed + i * (i + 1) / 2;
-    const long long re = r1 < i + 1 ? r1 : i + 1;
-    for (long long j = r0 + threadIdx.x; j < re; j += blockDim.x) d[j] = s[j];
-  }
-}
 __global__ void unpack_upper_kernel(long long n, const double* packed, double* dst, long long ldd) {
   for (long long i = blockIdx.x; i < n; i += gridDim.x) {
     const double* s = packed + i * (i + 1) / 2;
@@ -228,15 +216,6 @@ capital_status_t pack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const 
   const int tli = ctx->tl_begin(st, 8, 3, (double)col_begin, (double)col_end);
   pack_upper_kernel<<<(int)(cols < ctx->num_sms * 8 ? cols : ctx->num_sms * 8), 256, 0, st>>>(col_begin, col_end, src, lds, packed, zero_diag);
   ctx->tl_end(st, tli);
-  LAUNCH_CHECK();
-  return CAPITAL_OK;
-}
-capital_status_t emit_block_packed(capital_ctx* ctx, cudaStream_t st, const double* src, int64_t lds, double* packed, int64_t r0, int64_t r1,
-                                   int64_t c0, int64_t c1, int ctas) {
-  if (c1 <= c0 || r1 <= r0) return CAPITAL_OK;
-  const int64_t cols = c1 - c0;
-  if (ctas < 1) ctas = 1;
-  emit_block_packed_kernel<<<(int)(cols < ctas ? cols : ctas), 512, 0, st>>>(src, lds, packed, r0, r1, c0, c1);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

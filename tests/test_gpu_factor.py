@@ -142,34 +142,6 @@ def test_cholinv_streamed_host_path_equals_resident_path(topo, n, ci):
     assert cb.cholinv.residual(A, dev, topo) <= 1e-12
 
 
-@pytest.mark.skipif(not os.environ.get("CAPITAL_TEST_EXPERIMENTAL"), reason="opt-in: block-wise zero-copy host output (CAPITAL_ZC_OUT), not validated yet")
-@pytest.mark.parametrize("n,ci,depth", [(4096, 1, 3), (8192, 0, 3), (9088, 1, 2), (16384, 0, 3), (2048, 1, 0)])
-def test_cholinv_blockwise_host_output_equals_resident_path(n, ci, depth, monkeypatch):
-    """CAPITAL_ZC_OUT=1: every block of R / Rinv is stored into the pinned packed outputs as soon as it is final; the blocks must tile
-    the packed triangles exactly (outputs pre-filled with NaN) and carry the same bits as the resident path."""
-    monkeypatch.setenv("CAPITAL_ZC_OUT", "1")
-    monkeypatch.setenv("CAPITAL_ZC_DEPTH", str(depth))
-    cb.topo.release_contexts()  # the switches are read when a context is created
-    try:
-        t = cb.topo.square(1, 0, 1)
-        A = cb.matrix(n, n, 1, 1).distribute_symmetric(t)
-        dev = cb.cholinv.info(ci, 1, -4, "U")
-        cb.cholinv.factor(A, dev, t)
-        hostA = cb.matrix(n, n, 1, 1, data=A.data.cpu().pin_memory())
-        hst = cb.cholinv.info(ci, 1, -4, "U")
-        ctx = t.context()
-        for _ in range(2):
-            cnt = n * (n + 1) // 2
-            hst.R = torch.full((cnt,), float("nan"), dtype=torch.float64).pin_memory()
-            hst.Rinv = torch.full((cnt,), float("nan"), dtype=torch.float64).pin_memory()
-            ctx.reset_counters()
-            cb.cholinv.factor(hostA, hst, t)
-            assert ctx.counters().d2h_bytes == 2 * cnt * 8
-            assert torch.equal(hst.R, dev.R.cpu()) and torch.equal(hst.Rinv, dev.Rinv.cpu())
-    finally:
-        cb.topo.release_contexts()
-
-
 def test_cholinv_rejects_non_spd(topo):
     n = 256
     A = cb.matrix(n, n, 1, 1).distribute_symmetric(topo)
