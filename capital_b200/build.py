@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "_obj")
 LIB = os.path.join(HERE, "libcapital_b200.so")
-SOURCES = ["api.cu", "gemm_tn.cu", "leaf.cu", "layout.cu", "cholinv_local.cu", "dist.cu", "peer.cu", "gemm_tf32.cu"]
+SOURCES = ["api.cu", "gemm_tn.cu", "leaf.cu", "layout.cu", "cholinv_local.cu", "dist.cu", "peer.cu", "gemm_tf32.cu", "solve.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -dlcm=cg: plain global loads are cached in L2 only.  Buffers of the multi-GPU path are written by OTHER processes' copy engines and
 # kernels (peer DMA into mirror / gather slots, remote epilogue stores into exchange buffers and C replicas) and re-used every few

@@ -3,6 +3,7 @@
     args = cholinv.info(complete_inv, split, bc_mult_dim, 'U')      # cholinv.h:25-30
     cholinv.factor(A, args, topo)                                    # cholinv.hpp:6-28  -> args.R, args.Rinv
     R = cholinv.construct_R(args, topo)                              # cholinv.hpp:30-37 -> rect, zero lower
+    X = cholinv.solve(args, B, topo)                                 # A X = B from the factors (capital_cholinv_solve_f64)
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -78,3 +79,27 @@ def residual(A: matrix, args: info, topo) -> float:
                                                       _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
                                                       args.R.data_ptr(), C.byref(r)))
     return float(r.value)
+
+
+def solve(args: info, B: torch.Tensor, topo) -> torch.Tensor:
+    """A X = B with the factors of a previous `factor(A, args, topo)` (capital_cholinv_solve_f64).  B: float64, shape (n,) or (n, k),
+    on CUDA or on the host; the full right-hand side, the same on every rank of a grid.  Returns X with B's shape and device
+    (bit-identical on every rank)."""
+    if args.R is None or args.Rinv is None or args.global_dim <= 0:
+        raise ValueError("cholinv.solve: `args` holds no factors (run cholinv.factor first)")
+    if not isinstance(B, torch.Tensor) or B.dtype != torch.float64:
+        raise ValueError("cholinv.solve: B must be a float64 tensor")
+    if B.dim() not in (1, 2) or B.shape[0] != args.global_dim or B.numel() == 0:
+        raise ValueError(f"cholinv.solve: B must have shape ({args.global_dim},) or ({args.global_dim}, k), got {tuple(B.shape)}")
+    L = args.local_dim
+    if args.R.numel() != args.Rinv.numel() or args.Rinv.numel() != (L * (L + 1) // 2 if args.serialize else L * L):
+        raise ValueError("cholinv.solve: args.R / args.Rinv do not hold factors of the local dimension args.local_dim")
+    n = args.global_dim
+    k = 1 if B.dim() == 1 else B.shape[1]
+    Bc = B.contiguous() if B.dim() == 1 else B.t().contiguous()  # column-major n x k, ld n
+    Xc = torch.empty_like(Bc)
+    ctx = topo.context()
+    cargs = args._c()
+    ctx.check(_lib.lib().capital_cholinv_solve_f64(ctx.handle, n, C.byref(cargs), _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
+                                                   args.R.data_ptr(), args.Rinv.data_ptr(), k, Bc.data_ptr(), n, Xc.data_ptr(), n))
+    return Xc if B.dim() == 1 else Xc.t().contiguous()

@@ -6,6 +6,7 @@
 #include "peer.cuh"
 #include <math.h>
 #include <stdlib.h>
+#include <algorithm>
 
 capital_status_t capital_ctx::workspace(const std::string& name, size_t bytes, void** out) {
   capital_ctx* ctx = this;
@@ -624,6 +625,68 @@ capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_
   CAP_CUDA(cudaMemcpyAsync(h, ctx->d_scalars, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CAP_CUDA(cudaStreamSynchronize(st));
   *residual = sqrt(h[0]) / sqrt(h[1]);  // util.hpp:51
+  return CAPITAL_OK;
+}
+
+// A X = B from the factor's outputs.  Rinv complete: X = Rinv (Rinv^T B), two passes over the triangle per panel.  Top-level Rinv12
+// skipped (complete_inv = 0 and the top node splits at s1): the block formula with R12 (the reference's cacqr::solve, cacqr.hpp:44-73)
+//   Y1 = Rinv11^T B1,  Y2 = Rinv22^T (B2 - R12^T Y1),  X2 = Rinv22 Y2,  X1 = Rinv11 (Y1 - R12 X2).
+capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                           const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
+                                           double* X, int64_t ldx) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!args || !Rinv_local || !B || !X || n <= 0 || nrhs < 1 || ldb < n || ldx < n || args->split <= 0 || args->dir != 'U' ||
+      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED)) {
+    ctx->set_error("cholinv::solve: invalid arguments (Rinv, B, X non-null, nrhs >= 1, ldb, ldx >= n, split > 0 and dir == 'U')");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  const capital_grid_t& g = ctx->grid;
+  if (g.size > 1) return dist_cholinv_solve(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx);
+  const int64_t L = n;
+  const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
+  const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::solve: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  const int64_t s1 = L >> args->split;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const size_t f_count = packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
+  const int64_t ldu = packed ? 0 : L;
+  cudaStream_t st = ctx->stream;
+  const double *dRi, *dR = nullptr, *dB;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
+  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
+  CAP_TRY(cap_stage_in(ctx, B, (size_t)ldb * (nrhs - 1) + n, "solve_B", &dB));
+  const bool x_host = !cap_is_device_ptr(X);
+  double* dX = X;
+  if (x_host) CAP_TRY(ctx->workspace("solve_X", (size_t)ldx * nrhs * 8, (void**)&dX));
+  double *T, *T2;  // panel intermediates, L x SOLVE_W
+  CAP_TRY(ctx->workspace("solve_T", (size_t)L * SOLVE_W * 8, (void**)&T));
+  CAP_TRY(ctx->workspace("solve_T2", (size_t)L * SOLVE_W * 8, (void**)&T2));
+  for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+    const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+    const double* Bp = dB + p0 * ldb;
+    double* Xp = dX + p0 * ldx;
+    //                 U    ldu  trans r0  r1  c0  c1  nrhs alpha P  pinc ldp   beta Cin     ldcin C   cinc ldc
+    if (!skipped) {
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, 0, L, 0, L, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L}));    // Y = Rinv^T B
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, 0, L, 0, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx}));  // X = Rinv Y
+    } else {
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, 0, s1, 0, s1, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L}));   // T1 = Y1
+      CAP_TRY(tri_apply(ctx, st, {dR, ldu, true, 0, s1, s1, L, w, -1.0, T, 1, L, 1.0, Bp, ldb, T2, 1, L}));       // T2_2 = B2 - R12^T Y1
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, s1, L, s1, L, w, 1.0, T2, 1, L, 0.0, nullptr, 0, T, 1, L}));    // T2 = Y2
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, s1, L, s1, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx})); // X2
+      CAP_TRY(tri_apply(ctx, st, {dR, ldu, false, 0, s1, s1, L, w, -1.0, Xp, 1, ldx, 1.0, T, L, T2, 1, L}));      // T2_1 = Y1 - R12 X2
+      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, 0, s1, 0, s1, w, 1.0, T2, 1, L, 0.0, nullptr, 0, Xp, 1, ldx})); // X1
+    }
+  }
+  if (x_host) {  // only the n rows of each column travel: the caller's rows n .. ldx stay untouched
+    CAP_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * 8, dX, (size_t)ldx * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
+    ctx->counters.d2h_bytes += n * nrhs * 8;
+    CAP_CUDA(cudaStreamSynchronize(st));
+  }
   return CAPITAL_OK;
 }
 

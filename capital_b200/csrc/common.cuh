@@ -206,6 +206,32 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
                                double* Ri, int64_t ldri, double* RiT, int64_t ldrit, bool complete_top, int64_t bc, int split,
                                const CholinvHooks* hooks = nullptr, bool allow_side = true);
 
+// ---- solve.cu ---------------------------------------------------------------------------------
+// C = beta Cin + alpha op(U[r0:r1, c0:c1]) P for one panel of nrhs <= SOLVE_W right-hand sides (op = T when `trans`).  U: upper
+// triangular, packed (ldu == 0, column i at i(i+1)/2) or rect (ld ldu); entries below the diagonal are never read.  Panel rows are
+// addressed by the factor index: P(k, w) at P[k pinc + w ldp], C(o, w) at C[o cinc + w ldc], Cin(o, w) at Cin[o cinc + w ldcin]
+// (Cin may be null, or C itself).  pinc / cinc > 1 gather / scatter the cyclic rows of a grid rank from a full-length vector.
+constexpr int SOLVE_W = 32;
+struct TriApply {
+  const double* U;
+  int64_t ldu;
+  bool trans;
+  int64_t r0, r1, c0, c1;
+  int64_t nrhs;
+  double alpha;
+  const double* P;
+  int64_t pinc, ldp;
+  double beta;
+  const double* Cin;
+  int64_t ldcin;
+  double* C;
+  int64_t cinc, ldc;
+};
+capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& a);
+// Out = S + Cin (Cin may be null) on a rows x w column-major panel
+capital_status_t panel_add(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t w, const double* S, int64_t lds, const double* Cin,
+                           int64_t ldcin, double* Out, int64_t ldo);
+
 static inline int64_t round_up(int64_t a, int64_t b) { return (a + b - 1) / b * b; }
 // Does cholinv::invoke split a node of (global = local, single GPU) size n, or is it the reference's base case (potrf + trtri of the
 // whole block, cholinv.hpp:93)?  Decides whether complete_inv == 0 skips an inverse block at all: a top-level base case always

@@ -1180,6 +1180,99 @@ capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, 
   return CAPITAL_OK;
 }
 
+// cholinv::solve on the grid.  B and X are full and replicated; rank (x, y, z) holds rows = y and columns = x (mod d) of the factor.
+// Every triangular product of the single-GPU solve (api.cu) becomes: apply the local window to the gathered rows of the input
+// (op T: rows = y, op N: rows = x), scatter the result into the rank's rows of a zeroed n x SOLVE_W partial (op T: rows = x, op N:
+// rows = y), and sum the partials over all ranks with peer_allreduce_sum, which adds them in rank order -- X is bit-identical
+// everywhere.  The c layers split each window's columns into shares of equal triangle area, so every factor element enters the sum
+// exactly once.
+capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                    const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
+                                    double* X, int64_t ldx) {
+  CAP_TRY(need_comm(ctx));
+  Dist D;
+  CAP_TRY(dist_setup(D, ctx, false));
+  CAP_TRY(cholinv_shape(D, n, args));
+  const capital_grid_t& g = D.g;
+  const int64_t L = D.L, d = g.d;
+  const bool skipped = args->complete_inv == 0 && node_splits(D, L);  // the factor's predicate (cholinv_run)
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::solve: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  const int64_t s1 = L >> D.split;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const size_t f_count = packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
+  const int64_t ldu = packed ? 0 : L;
+  cudaStream_t st = ctx->stream;
+  const double *dRi, *dR = nullptr, *dB;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
+  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
+  CAP_TRY(cap_stage_in(ctx, B, (size_t)ldb * (nrhs - 1) + n, "solve_B", &dB));
+  const bool x_host = !cap_is_device_ptr(X);
+  double* dX = X;
+  if (x_host) CAP_TRY(ctx->workspace("solve_X", (size_t)ldx * nrhs * 8, (void**)&dX));
+  double *T, *T2, *S;  // full-length panel intermediates and the partial, n x SOLVE_W
+  CAP_TRY(ctx->workspace("solve_T", (size_t)n * SOLVE_W * 8, (void**)&T));
+  CAP_TRY(ctx->workspace("solve_T2", (size_t)n * SOLVE_W * 8, (void**)&T2));
+  CAP_TRY(ctx->workspace("solve_S", (size_t)n * SOLVE_W * 8, (void**)&S));
+  // the all-reduce always sums whole n x SOLVE_W panels: its two slot sets then keep the same place from one call to the next
+  const int64_t count = n * SOLVE_W;
+  const size_t bytes = (size_t)2 * D.world * count * 8;
+  CAP_TRY(arena_prepare(ctx, bytes, "cholsolve:" + std::to_string(n)));
+  double* slots = (double*)D.P->arena;
+  CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
+  // this layer's share [ca, cb) of the window's columns: equal triangle area per layer, the same cut on every rank
+  auto share = [&](int64_t r0, int64_t r1, int64_t c0, int64_t c1, int64_t* ca, int64_t* cb) {
+    auto area = [&](int64_t i) { return std::max<int64_t>(0, std::min(i + 1, r1) - r0); };
+    int64_t total = 0;
+    for (int64_t i = c0; i < c1; i++) total += area(i);
+    std::vector<int64_t> edge(g.c + 1, c1);
+    edge[0] = c0;
+    int64_t acc = 0;
+    int zi = 1;
+    for (int64_t i = c0; i < c1 && zi < g.c; i++) {
+      while (zi < g.c && acc * g.c >= total * zi) edge[zi++] = i;
+      acc += area(i);
+    }
+    *ca = edge[g.z];
+    *cb = edge[g.z + 1];
+  };
+  // Out[global rows of the result block] = alpha op(U window) In + Cin, for a panel of w columns
+  auto step = [&](const double* U, bool trans, int64_t r0, int64_t r1, int64_t c0, int64_t c1, int64_t w, double alpha, const double* In,
+                  int64_t ldi, const double* Cin, int64_t ldcin, double* Out, int64_t ldo) -> capital_status_t {
+    CAP_CUDA(cudaMemsetAsync(S, 0, (size_t)count * 8, st));
+    int64_t ca, cb;
+    share(r0, r1, c0, c1, &ca, &cb);
+    const int64_t pin = trans ? g.y : g.x, pout = trans ? g.x : g.y;
+    if (cb > ca) CAP_TRY(tri_apply(ctx, st, {U, ldu, trans, r0, r1, ca, cb, w, alpha, In + pin, d, ldi, 0.0, nullptr, 0, S + pout, d, n}));
+    CAP_TRY(peer_allreduce_sum(ctx, st, S, count, slots));
+    const int64_t o0 = d * (trans ? c0 : r0), o1 = d * (trans ? c1 : r1);
+    return panel_add(ctx, st, o1 - o0, w, S + o0, n, Cin ? Cin + o0 : nullptr, ldcin, Out + o0, ldo);
+  };
+  for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+    const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+    const double* Bp = dB + p0 * ldb;
+    double* Xp = dX + p0 * ldx;
+    if (!skipped) {
+      CAP_TRY(step(dRi, true, 0, L, 0, L, w, 1.0, Bp, ldb, nullptr, 0, T, n));    // Y = Rinv^T B
+      CAP_TRY(step(dRi, false, 0, L, 0, L, w, 1.0, T, n, nullptr, 0, Xp, ldx));   // X = Rinv Y
+    } else {
+      CAP_TRY(step(dRi, true, 0, s1, 0, s1, w, 1.0, Bp, ldb, nullptr, 0, T, n));  // Y1
+      CAP_TRY(step(dR, true, 0, s1, s1, L, w, -1.0, T, n, Bp, ldb, T2, n));       // B2 - R12^T Y1
+      CAP_TRY(step(dRi, true, s1, L, s1, L, w, 1.0, T2, n, nullptr, 0, T, n));    // Y2
+      CAP_TRY(step(dRi, false, s1, L, s1, L, w, 1.0, T, n, nullptr, 0, Xp, ldx)); // X2
+      CAP_TRY(step(dR, false, 0, s1, s1, L, w, -1.0, Xp, ldx, T, n, T2, n));      // Y1 - R12 X2
+      CAP_TRY(step(dRi, false, 0, s1, 0, s1, w, 1.0, T2, n, nullptr, 0, Xp, ldx)); // X1
+    }
+  }
+  if (x_host) {
+    CAP_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * 8, dX, (size_t)ldx * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
+    ctx->counters.d2h_bytes += n * nrhs * 8;
+  }
+  return cap_check_info(ctx);
+}
+
 capital_status_t dist_summa_gemm_tn(capital_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha, const double* A_local,
                                     const double* B_local, double beta, double* C_local) {
   CAP_TRY(need_comm(ctx));

@@ -156,6 +156,20 @@ capital_status_t capital_cholinv_factor_f64(capital_ctx* ctx, const double* A_lo
 capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_local, int64_t n_global,
                                               capital_structure_t structure, const double* R_local, double* residual);
 
+/* cholesky::cholinv solve: A X = B with the outputs of capital_cholinv_factor_f64 (A = R^T R).  Collective on a grid: every rank calls
+ * it with the same n_global, args (the ones given to the factor), structure and nrhs.  R_local / Rinv_local: this rank's local blocks
+ * exactly as the factor wrote them (packed upper or rect).  B, X: the FULL n x nrhs right-hand side / solution, column-major,
+ * ldb, ldx >= n, replicated: the same B on every rank in, bit-identical X on every rank out.  X may alias B (ldx == ldb).
+ * R_local is read only when the top-level Rinv12 block was skipped (complete_inv = 0 and the top node splits); it may be NULL otherwise.
+ * Rinv complete: X = Rinv (Rinv^T B).  Rinv12 skipped (split n1): Y1 = Rinv11^T B1, Y2 = Rinv22^T (B2 - R12^T Y1), X2 = Rinv22 Y2,
+ * X1 = Rinv11 (Y1 - R12 X2).  The factor is read in place, one pass per product and panel of up to 32 right-hand sides; the result is
+ * deterministic (same inputs, same bits).  Host or device pointers.  One GPU: enqueued on the context stream, synchronous only when X
+ * is a host pointer.  Grid: synchronous; its all-reduce slots use the peer arena, so the next factor call re-clears the arena.
+ * CAPITAL_ERR_UNSUPPORTED when d does not divide n on a grid. */
+capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                           capital_structure_t structure, const double* R_local, const double* Rinv_local,
+                                           int64_t nrhs, const double* B, int64_t ldb, double* X, int64_t ldx);
+
 /* ---- CholeskyQR2 --------------------------------------------------------------------------- */
 /* qr::cacqr<SP,IP>::factor(A, args, topo) -- cacqr.hpp:217-248, on a topo::rect grid c x d x c.  num_iter: 1 = CQR, 2 = CQR2.
  *  1D (c == 1, d == size): invoke_1d :172-193, sweep_1d :5-29, Gram allreduce policy.h:78-85.  A_local: (m/d) x n rect, Q_local same
