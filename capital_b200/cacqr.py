@@ -3,6 +3,12 @@
     ci = cholinv.info(complete_inv, split, bc_mult_dim, 'U')
     args = cacqr.info(num_iter, ci)                 # 1 = CholeskyQR, 2 = CholeskyQR2   (cacqr.h:28-32)
     cacqr.factor(A, args, topo)                     # cacqr.hpp:217-248 -> args.Q (rect), args.R (packed upper)
+    Y = cacqr.apply_QT(B, args, topo)               # cacqr.h:55: Q^T B      (capital_cacqr_apply_qt_f64)
+    C = cacqr.apply_Q(Z, args, topo)                # cacqr.h:52: Q Z        (capital_cacqr_apply_q_f64)
+    X = cacqr.lstsq(args, B, topo)                  # argmin ||A X - B|| = R^-1 Q^T B   (capital_cacqr_lstsq_f64)
+
+apply_QT / apply_Q / lstsq run on one GPU and on the 1D row grid (topo.rect with c = 1).  B and C hold this rank's rows (the rows
+of A.data: shape (rows_local,) or (rows_local, k)); Y, Z and X are the full n-row right-hand sides, the same on every rank.
 """
 from __future__ import annotations
 import ctypes as C
@@ -20,6 +26,9 @@ class info:
         self.Q = None
         self.R = None
         self.n = 0
+        self.rows_local = 0
+        self.m_global = 0
+        self.n_global = 0
 
 
 def factor(A: matrix, args: info, topo):
@@ -35,6 +44,7 @@ def factor(A: matrix, args: info, topo):
         args.R = torch.empty(rcount, dtype=torch.float64, device=dev, pin_memory=pin)
     args.n = lc
     args.rows_local = A.num_rows_local
+    args.m_global, args.n_global = m, n
     cargs = args.cholesky_inverse_args._c()
     ctx.check(_lib.lib().capital_cacqr_factor_f64(ctx.handle, A.data.data_ptr(), m, n, args.num_iter, C.byref(cargs),
                                                   _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
@@ -57,3 +67,65 @@ def validate(A: matrix, args: info, topo):
                                                     args.Q.data_ptr(), _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
                                                     args.R.data_ptr(), C.byref(r), C.byref(o)))
     return float(r.value), float(o.value)
+
+
+def _check(name: str, args: info, T, rows: int, what: str) -> int:
+    """ValueError unless `args` holds factors and T is a float64 tensor of `rows` rows (1-D or 2-D); returns the column count."""
+    if args.Q is None or args.R is None or args.m_global <= 0 or args.n_global <= 0:
+        raise ValueError(f"cacqr.{name}: `args` holds no factors (run cacqr.factor first)")
+    if not isinstance(T, torch.Tensor) or T.dtype != torch.float64:
+        raise ValueError(f"cacqr.{name}: {what} must be a float64 tensor")
+    if T.dim() not in (1, 2) or T.shape[0] != rows or T.numel() == 0:
+        raise ValueError(f"cacqr.{name}: {what} must have shape ({rows},) or ({rows}, k), got {tuple(T.shape)}")
+    if args.Q.numel() != args.rows_local * args.n:
+        raise ValueError(f"cacqr.{name}: args.Q does not hold rows_local x n values")
+    return 1 if T.dim() == 1 else T.shape[1]
+
+
+def _colmajor(T: torch.Tensor) -> torch.Tensor:
+    return T.contiguous() if T.dim() == 1 else T.t().contiguous()
+
+
+def _result(Tc: torch.Tensor, dim: int) -> torch.Tensor:
+    return Tc if dim == 1 else Tc.t().contiguous()
+
+
+def apply_QT(B: torch.Tensor, args: info, topo) -> torch.Tensor:
+    """Q^T B (capital_cacqr_apply_qt_f64).  B: this rank's rows, (rows_local,) or (rows_local, k), float64, on CUDA or the host.
+    Returns Y with shape (n,) or (n, k) on B's device, bit-identical on every rank."""
+    k = _check("apply_QT", args, B, args.rows_local, "B")
+    Bc = _colmajor(B)
+    Yc = torch.empty((args.n_global,) if B.dim() == 1 else (k, args.n_global), dtype=torch.float64, device=B.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cacqr_apply_qt_f64(ctx.handle, args.m_global, args.n_global, args.Q.data_ptr(), k, Bc.data_ptr(),
+                                                    args.rows_local, Yc.data_ptr(), args.n_global))
+    return _result(Yc, B.dim())
+
+
+def apply_Q(Z: torch.Tensor, args: info, topo) -> torch.Tensor:
+    """Q Z (capital_cacqr_apply_q_f64).  Z: (n,) or (n, k), float64, the same on every rank.  Returns this rank's rows of Q Z,
+    (rows_local,) or (rows_local, k), on Z's device."""
+    k = _check("apply_Q", args, Z, args.n_global, "Z")
+    Zc = _colmajor(Z)
+    Cc = torch.empty((args.rows_local,) if Z.dim() == 1 else (k, args.rows_local), dtype=torch.float64, device=Z.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cacqr_apply_q_f64(ctx.handle, args.m_global, args.n_global, args.Q.data_ptr(), k, Zc.data_ptr(),
+                                                   args.n_global, Cc.data_ptr(), args.rows_local))
+    return _result(Cc, Z.dim())
+
+
+def lstsq(args: info, B: torch.Tensor, topo) -> torch.Tensor:
+    """argmin_X ||A X - B||_F = R^-1 Q^T B from the factors of `factor(A, args, topo)` (capital_cacqr_lstsq_f64).  B: this rank's
+    rows, (rows_local,) or (rows_local, k), float64, on CUDA or the host.  Returns X with shape (n,) or (n, k) on B's device,
+    bit-identical on every rank."""
+    k = _check("lstsq", args, B, args.rows_local, "B")
+    n = args.n_global
+    if args.R.numel() != (n * (n + 1) // 2 if args.serialize else n * n):
+        raise ValueError("cacqr.lstsq: args.R does not hold an n x n factor")
+    Bc = _colmajor(B)
+    Xc = torch.empty((n,) if B.dim() == 1 else (k, n), dtype=torch.float64, device=B.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cacqr_lstsq_f64(ctx.handle, args.m_global, n, args.Q.data_ptr(),
+                                                 _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT, args.R.data_ptr(), k,
+                                                 Bc.data_ptr(), args.rows_local, Xc.data_ptr(), n))
+    return _result(Xc, B.dim())

@@ -710,6 +710,40 @@ capital_status_t capital_cacqr_residual_f64(capital_ctx* ctx, const double* A_lo
   return dist_cacqr_residual(ctx, A_local, m, n, Q_local, rstruct, R_local, residual, orthogonality);
 }
 
+// Q^T B, R^-1 Q^T B and Q Z from the factor's outputs (dist.cu).  B_local / C_local: the rank's lr = ceil(m / d) rows; Y, X, Z: n x nrhs.
+capital_status_t capital_cacqr_apply_qt_f64(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, int64_t nrhs,
+                                            const double* B_local, int64_t ldb, double* Y, int64_t ldy) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!Q_local || !B_local || !Y || n <= 0 || m < n || nrhs < 1 || ldb < ceil_div(m, ctx->grid.d) || ldy < n) {
+    ctx->set_error("cacqr::apply_QT: invalid arguments (Q, B, Y non-null, m >= n > 0, nrhs >= 1, ldb >= ceil(m / d), ldy >= n)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  return dist_cacqr_apply_qt(ctx, m, n, Q_local, CAPITAL_RECT, nullptr, nrhs, B_local, ldb, Y, ldy);
+}
+capital_status_t capital_cacqr_apply_q_f64(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, int64_t nrhs,
+                                           const double* Z, int64_t ldz, double* C_local, int64_t ldc) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!Q_local || !Z || !C_local || n <= 0 || m < n || nrhs < 1 || ldz < n || ldc < ceil_div(m, ctx->grid.d)) {
+    ctx->set_error("cacqr::apply_Q: invalid arguments (Q, Z, C non-null, m >= n > 0, nrhs >= 1, ldz >= n, ldc >= ceil(m / d))");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  return dist_cacqr_apply_q(ctx, m, n, Q_local, nrhs, Z, ldz, C_local, ldc);
+}
+capital_status_t capital_cacqr_lstsq_f64(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, capital_structure_t rstruct,
+                                         const double* R_local, int64_t nrhs, const double* B_local, int64_t ldb, double* X, int64_t ldx) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!Q_local || !R_local || !B_local || !X || n <= 0 || m < n || nrhs < 1 || ldb < ceil_div(m, ctx->grid.d) || ldx < n ||
+      (rstruct != CAPITAL_RECT && rstruct != CAPITAL_UPPERTRI_PACKED)) {
+    ctx->set_error("cacqr::lstsq: invalid arguments (Q, R, B, X non-null, m >= n > 0, nrhs >= 1, ldb >= ceil(m / d), ldx >= n, "
+                   "R packed upper or rect)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  return dist_cacqr_apply_qt(ctx, m, n, Q_local, rstruct, R_local, nrhs, B_local, ldb, X, ldx);
+}
+
 // ---- SUMMA -----------------------------------------------------------------------------------
 capital_status_t capital_summa_gemm_tn_f64(capital_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha, const double* A_local,
                                            const double* B_local, double beta, double* C_local) {

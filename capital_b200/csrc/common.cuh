@@ -226,8 +226,13 @@ struct TriApply {
   int64_t ldcin;
   double* C;
   int64_t cinc, ldc;
+  bool full = false;  // a rect window read whole (no j <= i mask, no triangular k ranges): Q^T P and Q P for a tall rect Q (ldu > 0)
 };
 capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& a);
+// Y <- U[0:n, 0:n]^-1 Y in place for one panel of nrhs <= SOLVE_W right-hand sides (Y(k, w) at Y[k + w ldy]); U upper triangular,
+// packed (ldu == 0) or rect, entries below the diagonal never read.  Deterministic.
+capital_status_t tri_solve(capital_ctx* ctx, cudaStream_t st, const double* U, int64_t ldu, int64_t n, int64_t nrhs, double* Y,
+                           int64_t ldy);
 // Out = S + Cin (Cin may be null) on a rows x w column-major panel
 capital_status_t panel_add(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t w, const double* S, int64_t lds, const double* Cin,
                            int64_t ldcin, double* Out, int64_t ldo);

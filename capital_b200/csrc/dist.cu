@@ -1761,3 +1761,92 @@ capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, in
   *orthogonality = sqrt(h[2]) / sqrt((double)n * (double)n);
   return CAPITAL_OK;
 }
+
+// ---- cacqr::apply_QT / lstsq / apply_Q: one GPU and the 1D row grid ---------------------------------------------------------------
+namespace {
+// Q_local of capital_cacqr_factor_f64 is a block of whole rows only on one GPU and on the 1D row grid (c == 1, d == size)
+capital_status_t qr_rows_grid(capital_ctx* ctx, const char* what) {
+  const capital_grid_t& g = ctx->grid;
+  if (g.size == 1 || (g.c == 1 && g.d == g.size)) return CAPITAL_OK;
+  const std::string why = g.c != 1 ? "c = " + std::to_string(g.c) + " is not 1"
+                                   : "d = " + std::to_string(g.d) + " is not the grid size " + std::to_string(g.size);
+  ctx->set_error(std::string(what) + ": needs one GPU or the 1D row grid (c == 1, d == size); " + why);
+  return CAPITAL_ERR_UNSUPPORTED;
+}
+}  // namespace
+
+// Y = Q^T B and, when R_local is given, X = R^-1 Y (lstsq).  Each rank applies its rows of Q to its rows of B; on the grid the n x
+// SOLVE_W partials are summed by peer_allreduce_sum in rank order, so Y -- and X, since R is replicated -- is bit-identical on every
+// rank.  Every all-reduce of a call sums whole n x SOLVE_W panels, under the arena signature qrls:n.
+capital_status_t dist_cacqr_apply_qt(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, capital_structure_t rstruct,
+                                     const double* R_local, int64_t nrhs, const double* B_local, int64_t ldb, double* X, int64_t ldx) {
+  const char* what = R_local ? "cacqr::lstsq" : "cacqr::apply_QT";
+  CAP_TRY(qr_rows_grid(ctx, what));
+  CAP_TRY(need_comm(ctx));
+  const capital_grid_t& g = ctx->grid;
+  const bool grid = g.size > 1;
+  const int64_t lr = ceil_div(m, g.d);
+  cudaStream_t st = ctx->stream;
+  const bool packed = rstruct == CAPITAL_UPPERTRI_PACKED;
+  const double *dQ, *dB, *dR = nullptr;
+  CAP_TRY(cap_stage_in(ctx, Q_local, (size_t)lr * n, "lsq_Q", &dQ));
+  CAP_TRY(cap_stage_in(ctx, B_local, (size_t)ldb * (nrhs - 1) + lr, "lsq_B", &dB));
+  if (R_local) CAP_TRY(cap_stage_in(ctx, R_local, packed ? (size_t)n * (n + 1) / 2 : (size_t)n * n, "lsq_R", &dR));
+  const bool x_host = !cap_is_device_ptr(X);
+  double* dX = X;
+  if (x_host) CAP_TRY(ctx->workspace("lsq_X", (size_t)ldx * nrhs * 8, (void**)&dX));
+  const int64_t count = n * SOLVE_W;
+  double *S = nullptr, *slots = nullptr;
+  if (grid) {
+    CAP_TRY(ctx->workspace("lsq_S", (size_t)count * 8, (void**)&S));
+    CAP_CUDA(cudaMemsetAsync(S, 0, (size_t)count * 8, st));  // columns past a narrow last panel are summed too
+    CAP_TRY(arena_prepare(ctx, (size_t)2 * g.size * count * 8, "qrls:" + std::to_string(n)));
+    slots = (double*)peer_of(ctx)->arena;
+    CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
+  }
+  for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+    const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+    double* Xp = dX + p0 * ldx;
+    double* Y = grid ? S : Xp;
+    const int64_t ldy = grid ? n : ldx;
+    //                          U   ldu  trans r0  r1  c0  c1  nrhs alpha P               pinc ldp  beta Cin      ldcin C  cinc ldc  full
+    CAP_TRY(tri_apply(ctx, st, {dQ, lr, true, 0, lr, 0, n, w, 1.0, dB + p0 * ldb, 1, ldb, 0.0, nullptr, 0, Y, 1, ldy, true}));
+    if (grid) {
+      CAP_TRY(peer_allreduce_sum(ctx, st, S, count, slots));
+      CAP_TRY(panel_add(ctx, st, n, w, S, n, nullptr, 0, Xp, ldx));
+    }
+    if (dR) CAP_TRY(tri_solve(ctx, st, dR, packed ? 0 : n, n, w, Xp, ldx));
+  }
+  if (x_host) {  // only the n rows of each column travel: the caller's rows n .. ldx stay untouched
+    CAP_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * 8, dX, (size_t)ldx * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
+    ctx->counters.d2h_bytes += n * nrhs * 8;
+  }
+  if (grid) return cap_check_info(ctx);
+  if (x_host) CAP_CUDA(cudaStreamSynchronize(st));
+  return CAPITAL_OK;
+}
+
+// C_local = Q_local Z: each rank's rows of Q Z need only its own rows of Q -- no communication
+capital_status_t dist_cacqr_apply_q(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, int64_t nrhs, const double* Z,
+                                    int64_t ldz, double* C_local, int64_t ldc) {
+  CAP_TRY(qr_rows_grid(ctx, "cacqr::apply_Q"));
+  const int64_t lr = ceil_div(m, ctx->grid.d);
+  cudaStream_t st = ctx->stream;
+  const double *dQ, *dZ;
+  CAP_TRY(cap_stage_in(ctx, Q_local, (size_t)lr * n, "lsq_Q", &dQ));
+  CAP_TRY(cap_stage_in(ctx, Z, (size_t)ldz * (nrhs - 1) + n, "lsq_Z", &dZ));
+  const bool c_host = !cap_is_device_ptr(C_local);
+  double* dC = C_local;
+  if (c_host) CAP_TRY(ctx->workspace("lsq_C", (size_t)ldc * nrhs * 8, (void**)&dC));
+  for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+    const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+    //                          U   ldu  trans  r0  r1  c0  c1  nrhs alpha P               pinc ldp  beta Cin      ldcin C               cinc ldc  full
+    CAP_TRY(tri_apply(ctx, st, {dQ, lr, false, 0, lr, 0, n, w, 1.0, dZ + p0 * ldz, 1, ldz, 0.0, nullptr, 0, dC + p0 * ldc, 1, ldc, true}));
+  }
+  if (c_host) {  // only the lr rows of each column travel
+    CAP_CUDA(cudaMemcpy2DAsync(C_local, (size_t)ldc * 8, dC, (size_t)ldc * 8, (size_t)lr * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
+    ctx->counters.d2h_bytes += lr * nrhs * 8;
+    CAP_CUDA(cudaStreamSynchronize(st));
+  }
+  return CAPITAL_OK;
+}

@@ -13,6 +13,10 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
                                     double* X, int64_t ldx);
 capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, int num_iter,
                                    const capital_cholinv_args_t* ci_args, capital_structure_t rstruct, double* Q_local, double* R_local);
+capital_status_t dist_cacqr_apply_qt(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, capital_structure_t rstruct,
+                                     const double* R_local, int64_t nrhs, const double* B_local, int64_t ldb, double* X, int64_t ldx);
+capital_status_t dist_cacqr_apply_q(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, int64_t nrhs, const double* Z,
+                                    int64_t ldz, double* C_local, int64_t ldc);
 capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, const double* Q_local,
                                      capital_structure_t rstruct, const double* R_local, double* residual, double* orthogonality);
 

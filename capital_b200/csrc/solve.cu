@@ -9,6 +9,9 @@
 // A triangle makes the owned blocks' k extents very uneven, so the k range of every block is cut into chunks of TA_KC tiles, one
 // CTA each, longest blocks first; stage 1 writes one partial per chunk, stage 2 adds the chunks of a block in chunk order and
 // applies alpha, beta.  No atomics anywhere: the same inputs give the same bits (the grid solve relies on it).
+//
+// FULL windows (cacqr::apply_QT / apply_Q / lstsq): the same kernel without the j <= i mask and with k over the whole other extent, so
+// a tall rect Q is read once for Q^T P (op T) or Q P (op N).  The substitution Y <- R^-1 Y of lstsq is tri_solve, at the end.
 #include "common.cuh"
 #include <algorithm>
 
@@ -31,10 +34,12 @@ struct TriDev {
 };
 
 // k range of owned block [olo, ohi): op T owns columns, k runs over the rows j <= i of the window; op N owns rows, k over the
-// columns i >= j
+// columns i >= j.  FULL (a rect, non-triangular window): k runs over the whole other extent
+template <bool FULL = false>
 __host__ __device__ inline void k_range(bool trans, int64_t r0, int64_t r1, int64_t c0, int64_t c1, int64_t olo, int64_t ohi,
                                         int64_t* klo, int64_t* khi) {
-  if (trans) { *klo = r0; *khi = r1 < ohi ? r1 : ohi; }
+  if (FULL) { *klo = trans ? r0 : c0; *khi = trans ? r1 : c1; }
+  else if (trans) { *klo = r0; *khi = r1 < ohi ? r1 : ohi; }
   else { *klo = c0 > olo ? c0 : olo; *khi = c1; }
 }
 __host__ __device__ inline int64_t n_chunks(int64_t klo, int64_t khi) {
@@ -42,7 +47,7 @@ __host__ __device__ inline int64_t n_chunks(int64_t klo, int64_t khi) {
   return (tiles + TA_KC - 1) / TA_KC;
 }
 
-template <int W, bool TRANS>
+template <int W, bool TRANS, bool FULL = false>
 __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
   constexpr int WG = W >= 4 ? 4 : 1;  // w groups (each owns WPT right-hand sides)
   constexpr int KG = 4 / WG;           // k groups (narrow panels split k instead, summed in group order at the end)
@@ -58,7 +63,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
   const int64_t o0 = TRANS ? a.c0 : a.r0, o1 = TRANS ? a.c1 : a.r1;
   const int64_t olo = o0 + b * TT, ohi = o1 < olo + TT ? o1 : olo + TT;
   int64_t klo, khi;
-  k_range(TRANS, a.r0, a.r1, a.c0, a.c1, olo, ohi, &klo, &khi);
+  k_range<FULL>(TRANS, a.r0, a.r1, a.c0, a.c1, olo, ohi, &klo, &khi);
   const int64_t ktiles = khi > klo ? (khi - klo + TT - 1) / TT : 0;
   const int64_t t0 = (int64_t)blockIdx.x * TA_KC, t1 = ktiles < t0 + TA_KC ? ktiles : t0 + TA_KC;
   if (t0 >= t1) return;
@@ -78,7 +83,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
 #pragma unroll
     for (int it = 0; it < TA_PER; it++) {
       double v = 0.0;
-      if (row_ok && i < iend && j <= i) v = col[j];
+      if (row_ok && i < iend && (FULL || j <= i)) v = col[j];
       ur[it] = v;
       col += packed ? 4 * i + 10 : 4 * a.ldu;  // start of column i + 4
       i += 4;
@@ -166,6 +171,7 @@ struct TriFin {
 };
 
 // C(o, w) = alpha * (sum of the block's chunk partials, in chunk order) + beta * Cin(o, w)
+template <bool FULL = false>
 __global__ void tri_finish_kernel(TriFin f) {
   const int64_t total = f.olen * f.nrhs;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
@@ -173,7 +179,7 @@ __global__ void tri_finish_kernel(TriFin f) {
     const int64_t b = orel / TT, oo = orel % TT;
     const int64_t olo = f.o0 + b * TT, ohi = (f.o0 + f.olen) < olo + TT ? f.o0 + f.olen : olo + TT;
     int64_t klo, khi;
-    k_range(f.trans, f.r0, f.r1, f.c0, f.c1, olo, ohi, &klo, &khi);
+    k_range<FULL>(f.trans, f.r0, f.r1, f.c0, f.c1, olo, ohi, &klo, &khi);
     const int64_t nch = n_chunks(klo, khi);
     double s = 0.0;
     for (int64_t c = 0; c < nch; c++) s += f.part[((b * f.cmax + c) * TT + oo) * f.w + w];
@@ -184,34 +190,72 @@ __global__ void tri_finish_kernel(TriFin f) {
   }
 }
 
-template <int W, bool TRANS>
+// Stage 2 for a full window whose k range is long (Q^T B: the k index runs over the rows of a tall Q, about a thousand chunks at
+// 2^20 rows): one warp per output, lane l adds chunks l, l + 32, ... in order, then a fixed butterfly adds the lanes -- still the
+// same bits for the same inputs
+__global__ void full_finish_kernel(TriFin f) {
+  const int lane = threadIdx.x & 31;
+  const int64_t total = f.olen * f.nrhs;
+  int64_t klo, khi;
+  k_range<true>(f.trans, f.r0, f.r1, f.c0, f.c1, 0, 0, &klo, &khi);
+  const int64_t nch = n_chunks(klo, khi);
+  const int64_t warps = (int64_t)gridDim.x * blockDim.x / 32;
+  for (int64_t idx = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32; idx < total; idx += warps) {
+    const int64_t orel = idx % f.olen, w = idx / f.olen;
+    const int64_t b = orel / TT, oo = orel % TT;
+    double s = 0.0;
+    for (int64_t c = lane; c < nch; c += 32) s += f.part[((b * f.cmax + c) * TT + oo) * f.w + w];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) {
+      const int64_t o = f.o0 + orel;
+      double v = f.alpha * s;
+      if (f.Cin) v += f.beta * f.Cin[o * f.cinc + w * f.ldcin];
+      f.C[o * f.cinc + w * f.ldc] = v;
+    }
+  }
+}
+
+template <int W, bool TRANS, bool FULL>
 capital_status_t launch_w(capital_ctx* ctx, cudaStream_t st, const TriDev& a, dim3 grid) {
   constexpr int PP = W == 1 ? 1 : W + 2;
   const size_t smem = (size_t)(TT * (TT + 1) + TT * PP) * 8;
-  CAP_CUDA(cudaFuncSetAttribute(tri_apply_kernel<W, TRANS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  tri_apply_kernel<W, TRANS><<<grid, TA_THREADS, smem, st>>>(a);
+  CAP_CUDA(cudaFuncSetAttribute(tri_apply_kernel<W, TRANS, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  tri_apply_kernel<W, TRANS, FULL><<<grid, TA_THREADS, smem, st>>>(a);
   CAP_CUDA(cudaGetLastError());
   return CAPITAL_OK;
 }
 
-template <bool TRANS>
+template <bool TRANS, bool FULL>
 capital_status_t launch_op(capital_ctx* ctx, cudaStream_t st, int w, const TriDev& a, dim3 grid) {
   switch (w) {
-    case 1: return launch_w<1, TRANS>(ctx, st, a, grid);
-    case 2: return launch_w<2, TRANS>(ctx, st, a, grid);
-    case 4: return launch_w<4, TRANS>(ctx, st, a, grid);
-    case 8: return launch_w<8, TRANS>(ctx, st, a, grid);
-    case 16: return launch_w<16, TRANS>(ctx, st, a, grid);
-    default: return launch_w<32, TRANS>(ctx, st, a, grid);
+    case 1: return launch_w<1, TRANS, FULL>(ctx, st, a, grid);
+    case 2: return launch_w<2, TRANS, FULL>(ctx, st, a, grid);
+    case 4: return launch_w<4, TRANS, FULL>(ctx, st, a, grid);
+    case 8: return launch_w<8, TRANS, FULL>(ctx, st, a, grid);
+    case 16: return launch_w<16, TRANS, FULL>(ctx, st, a, grid);
+    default: return launch_w<32, TRANS, FULL>(ctx, st, a, grid);
   }
 }
+
+constexpr int64_t TA_MAX_BLOCKS = 65535;  // owned blocks per launch (grid.y)
 
 }  // namespace
 
 capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x) {
   if (x.nrhs < 1 || x.nrhs > SOLVE_W) { ctx->set_error("tri_apply: 1 <= nrhs <= SOLVE_W"); return CAPITAL_ERR_INVALID; }
+  if (x.full && x.ldu == 0) { ctx->set_error("tri_apply: a full window needs rect storage"); return CAPITAL_ERR_INVALID; }
   const int64_t o0 = x.trans ? x.c0 : x.r0, o1 = x.trans ? x.c1 : x.r1;
   if (o1 <= o0) return CAPITAL_OK;
+  if (ceil_div(o1 - o0, TT) > TA_MAX_BLOCKS) {  // owned rows (columns) are independent: one launch per slab of them
+    for (int64_t s0 = o0; s0 < o1; s0 += TA_MAX_BLOCKS * TT) {
+      TriApply y = x;
+      (x.trans ? y.c0 : y.r0) = s0;
+      (x.trans ? y.c1 : y.r1) = std::min(o1, s0 + TA_MAX_BLOCKS * TT);
+      CAP_TRY(tri_apply(ctx, st, y));
+    }
+    return CAPITAL_OK;
+  }
   int w = 1;
   while (w < x.nrhs) w *= 2;  // smallest instantiated panel width that holds the panel
   const int64_t nob = ceil_div(o1 - o0, TT);
@@ -220,7 +264,8 @@ capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x)
   for (int64_t b : {(int64_t)0, nob - 1}) {
     const int64_t olo = o0 + b * TT, ohi = std::min(o1, olo + TT);
     int64_t klo, khi;
-    k_range(x.trans, x.r0, x.r1, x.c0, x.c1, olo, ohi, &klo, &khi);
+    if (x.full) k_range<true>(x.trans, x.r0, x.r1, x.c0, x.c1, olo, ohi, &klo, &khi);
+    else k_range(x.trans, x.r0, x.r1, x.c0, x.c1, olo, ohi, &klo, &khi);
     cmax = std::max(cmax, n_chunks(klo, khi));
   }
   double* part = nullptr;
@@ -228,14 +273,20 @@ capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x)
     CAP_TRY(ctx->workspace("solve_part", (size_t)nob * cmax * TT * w * 8, (void**)&part));
     TriDev a{x.U, x.ldu, x.r0, x.r1, x.c0, x.c1, (int)x.nrhs, x.P, x.pinc, x.ldp, part, nob, cmax};
     const dim3 grid((unsigned)cmax, (unsigned)nob);
-    if (x.trans) CAP_TRY(launch_op<true>(ctx, st, w, a, grid));
-    else CAP_TRY(launch_op<false>(ctx, st, w, a, grid));
+    auto launch = x.full ? (x.trans ? launch_op<true, true> : launch_op<false, true>) : (x.trans ? launch_op<true, false> : launch_op<false, false>);
+    CAP_TRY(launch(ctx, st, w, a, grid));
     ctx->counters.kernel_launches++;
   }
   TriFin f{x.trans, x.r0, x.r1, x.c0, x.c1, o0, o1 - o0, (int)x.nrhs, w, part, cmax, x.alpha, x.beta, x.Cin, x.ldcin, x.C, x.cinc, x.ldc};
   const int64_t total = (o1 - o0) * x.nrhs;
-  const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), 4 * (int64_t)ctx->num_sms);
-  tri_finish_kernel<<<blocks, 256, 0, st>>>(f);
+  if (x.full && cmax > 32) {
+    const int blocks = (int)std::min<int64_t>(ceil_div(total * 32, 256), 16 * (int64_t)ctx->num_sms);
+    full_finish_kernel<<<blocks, 256, 0, st>>>(f);
+  } else {
+    const int blocks = (int)std::min<int64_t>(ceil_div(total, 256), 4 * (int64_t)ctx->num_sms);
+    if (x.full) tri_finish_kernel<true><<<blocks, 256, 0, st>>>(f);
+    else tri_finish_kernel<<<blocks, 256, 0, st>>>(f);
+  }
   CAP_CUDA(cudaGetLastError());
   ctx->counters.kernel_launches++;
   return CAPITAL_OK;
@@ -261,5 +312,90 @@ capital_status_t panel_add(capital_ctx* ctx, cudaStream_t st, int64_t rows, int6
   panel_add_kernel<<<blocks, 256, 0, st>>>(rows, w, S, lds, Cin, ldcin, Out, ldo);
   CAP_CUDA(cudaGetLastError());
   ctx->counters.kernel_launches++;
+  return CAPITAL_OK;
+}
+
+// ---- triangular substitution: Y <- U^-1 Y ------------------------------------------------------------------------------------
+// Blocked from the bottom right in diagonal blocks of TS columns.  Each diagonal block is solved by one CTA: the block's triangle is
+// staged in shared memory (packed, column c at c(c+1)/2, with the reciprocals of its diagonal), one warp per right-hand side holds
+// the block's rows of its column in registers (row 32 s + lane in slot s), and back substitution runs warp-synchronously -- the
+// solved value is broadcast by shuffle, and no block barrier sits in the chain.  The rows above the block are then updated by tri_apply (op N, alpha = -1): that window
+// lies wholly above the diagonal, and the panel rows it reads are not the rows it writes.
+namespace {
+constexpr int TS = 128;
+constexpr int TS_SLOTS = TS / 32;
+constexpr int TS_THREADS = 1024;  // 32 warps: up to SOLVE_W right-hand sides, and all of them stage the triangle
+
+struct SolveDev {
+  const double* U;
+  int64_t ldu;  // 0: packed
+  int64_t b0, b1;
+  int nrhs;
+  double* Y;
+  int64_t ldy;
+};
+
+__global__ void __launch_bounds__(TS_THREADS) tri_block_solve_kernel(SolveDev a) {
+  extern __shared__ double Ts[];       // the triangle, packed
+  __shared__ double dinv[TS];          // reciprocals of its diagonal: the chain multiplies
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nb = (int)(a.b1 - a.b0);
+  const bool packed = a.ldu == 0;
+  // staging: every thread walks the nb x nb square with many independent loads in flight, rows of a column on consecutive threads
+#pragma unroll 8
+  for (int e = threadIdx.x; e < nb * nb; e += TS_THREADS) {
+    const int c = e / nb, r = e - c * nb;
+    if (r <= c) {
+      const int64_t i = a.b0 + c;
+      const double v = a.U[(packed ? i * (i + 1) / 2 : i * a.ldu) + a.b0 + r];
+      Ts[c * (c + 1) / 2 + r] = v;
+      if (r == c) dinv[c] = 1.0 / v;
+    }
+  }
+  const bool active = warp < a.nrhs;
+  double* yc = a.Y + (int64_t)warp * a.ldy + a.b0;
+  double y[TS_SLOTS];
+#pragma unroll
+  for (int s = 0; s < TS_SLOTS; s++) {
+    const int r = 32 * s + lane;
+    y[s] = active && r < nb ? yc[r] : 0.0;
+  }
+  __syncthreads();
+  if (!active) return;
+#pragma unroll
+  for (int s = TS_SLOTS - 1; s >= 0; s--) {
+    if (32 * s >= nb) continue;
+    for (int q = 31; q >= 0; q--) {
+      const int i = 32 * s + q;
+      if (i >= nb) continue;
+      const double* ci = Ts + i * (i + 1) / 2;
+      const double x = __shfl_sync(0xffffffffu, y[s], q) * dinv[i];
+      if (lane == q) y[s] = x;
+#pragma unroll
+      for (int s2 = 0; s2 <= s; s2++)
+        if (s2 < s || lane < q) y[s2] = fma(-ci[32 * s2 + lane], x, y[s2]);
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < TS_SLOTS; s++) {
+    const int r = 32 * s + lane;
+    if (r < nb) yc[r] = y[s];
+  }
+}
+}  // namespace
+
+capital_status_t tri_solve(capital_ctx* ctx, cudaStream_t st, const double* U, int64_t ldu, int64_t n, int64_t nrhs, double* Y,
+                           int64_t ldy) {
+  if (nrhs < 1 || nrhs > SOLVE_W) { ctx->set_error("tri_solve: 1 <= nrhs <= SOLVE_W"); return CAPITAL_ERR_INVALID; }
+  if (n <= 0) return CAPITAL_OK;
+  CAP_CUDA(cudaFuncSetAttribute(tri_block_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TS * (TS + 1) / 2 * 8));
+  for (int64_t b0 = (n - 1) / TS * TS; b0 >= 0; b0 -= TS) {
+    const int64_t b1 = std::min(n, b0 + TS), nb = b1 - b0;
+    tri_block_solve_kernel<<<1, TS_THREADS, (size_t)nb * (nb + 1) / 2 * 8, st>>>(SolveDev{U, ldu, b0, b1, (int)nrhs, Y, ldy});
+    CAP_CUDA(cudaGetLastError());
+    ctx->counters.kernel_launches++;
+    //                           U  ldu  trans r0  r1  c0  c1  nrhs  alpha P  pinc ldp  beta Cin ldcin C  cinc ldc
+    if (b0 > 0) CAP_TRY(tri_apply(ctx, st, {U, ldu, false, 0, b0, b0, b1, nrhs, -1.0, Y, 1, ldy, 1.0, Y, ldy, Y, 1, ldy}));
+  }
   return CAPITAL_OK;
 }

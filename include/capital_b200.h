@@ -186,6 +186,28 @@ capital_status_t capital_cacqr_factor_f64(capital_ctx* ctx, const double* A_loca
 capital_status_t capital_cacqr_residual_f64(capital_ctx* ctx, const double* A_local, int64_t m_global, int64_t n_global,
                                             const double* Q_local, capital_structure_t r_structure,
                                             const double* R_local, double* residual, double* orthogonality);
+/* qr::cacqr apply_QT / apply_Q (cacqr.h:52,55) and least squares, from the outputs of capital_cacqr_factor_f64 on one GPU or the 1D
+ * row grid (c == 1, d == size); other grids: CAPITAL_ERR_UNSUPPORTED.  Collective on the grid: every rank calls with the same
+ * m_global, n_global, nrhs (and r_structure).  Q_local, R_local: exactly as the factor wrote them -- Q_local lr x n with
+ * lr = ceil(m/d) and leading dimension lr; R_local packed upper or rect, replicated.  B_local / C_local: lr x nrhs, column-major,
+ * ldb / ldc >= lr, holding the rows this rank's A_local holds (global row gy at local row gy / d on rank gy mod d).  Where d does
+ * not divide m, the pad rows of Q are zero, so finite pad rows of B contribute nothing.  Y, Z, X: full n x nrhs, column-major,
+ * ldy / ldz / ldx >= n.  Right-hand sides go in panels of 32; each product reads Q once per panel, in place.  Only the rows of an
+ * output are written (rows n .. ldx, lr .. ldc stay untouched).  Host or device pointers.  Results are deterministic.  One GPU:
+ * enqueued on the context stream, synchronous only for a host output.  Grid: apply_QT and lstsq are synchronous; their all-reduce
+ * slots use the peer arena, so the next factor call re-clears the arena.  CAPITAL_ERR_INVALID: a NULL pointer, nrhs < 1, m < n, a
+ * leading dimension too small or a bad structure. */
+/* Y = Q^T B.  Y: full n x nrhs, replicated, bit-identical on every rank. */
+capital_status_t capital_cacqr_apply_qt_f64(capital_ctx* ctx, int64_t m_global, int64_t n_global, const double* Q_local,
+                                            int64_t nrhs, const double* B_local, int64_t ldb, double* Y, int64_t ldy);
+/* C_local = Q_local Z.  Z: full n x nrhs, the same on every rank.  No communication. */
+capital_status_t capital_cacqr_apply_q_f64(capital_ctx* ctx, int64_t m_global, int64_t n_global, const double* Q_local,
+                                           int64_t nrhs, const double* Z, int64_t ldz, double* C_local, int64_t ldc);
+/* X = argmin ||A X - B||_F = R^-1 (Q^T B): apply_QT, then triangular substitution with R (blocked, R read in place, entries below
+ * the diagonal never read).  X: full n x nrhs, replicated, bit-identical on every rank. */
+capital_status_t capital_cacqr_lstsq_f64(capital_ctx* ctx, int64_t m_global, int64_t n_global, const double* Q_local,
+                                         capital_structure_t r_structure, const double* R_local, int64_t nrhs,
+                                         const double* B_local, int64_t ldb, double* X, int64_t ldx);
 
 /* ---- SUMMA ------------------------------------------------------------------------------------ */
 /* matmult::summa::invoke(A, B, C, topo, gemm{Trans, NoTrans, alpha, beta}) -- summa.hpp:6-44 in the T*N form the validators
