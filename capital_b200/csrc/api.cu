@@ -147,9 +147,10 @@ capital_status_t hostio_left_done(void* user, cudaStream_t st, int64_t col_end, 
   // miss the off-diagonal inverse blocks of the right-spine ancestors, computed after their right children)
   const bool rinv_too = depth == 0 || (depth == 1 && io->rinv_streams && io->rinv_cols_out == c0);
   const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = (size_t)col_end * (col_end + 1) / 2 - off;
-  // packing is HBM-bound filler work: it goes to the low-priority stream (joined before cholinv_local returns), not to the chain
-  // (host callers keep it on the chain: the D2H of the range should start right away, not behind queued deferred work)
-  cudaStream_t ps = (ctx->side && !ctx->no_overlap && !io->hR && !io->hRinv) ? ctx->side : st;
+  // packing is HBM-bound filler work: it goes to a low-priority stream of its own (joined through e_out after the recursion), not
+  // to the chain, nor in front of the deferred far updates (the top-level one would wait for it).  Host callers keep it on the chain:
+  // the D2H of the range should start right away.
+  cudaStream_t ps = (!ctx->no_overlap && !io->hR && !io->hRinv) ? ctx->copy_out : st;
   cudaEvent_t e;
   if (ps != st) {
     CAP_TRY(io_event(ctx, &e));
@@ -160,7 +161,13 @@ capital_status_t hostio_left_done(void* user, cudaStream_t st, int64_t col_end, 
   if (rinv_too) CAP_TRY(pack_upper(ctx, ps, io->L, io->Ri, io->ld, io->dRinv, 0, c0, col_end));
   io->cols_out = col_end;
   if (rinv_too) io->rinv_cols_out = col_end;
-  if (!io->hR && !io->hRinv) return CAPITAL_OK;  // device outputs: nothing to copy out
+  if (!io->hR && !io->hRinv) {  // device outputs: nothing to copy out
+    if (ps != st) {
+      CAP_TRY(io_event(ctx, &io->e_out));
+      CAP_CUDA(cudaEventRecord(io->e_out, ps));
+    }
+    return CAPITAL_OK;
+  }
   CAP_TRY(io_event(ctx, &e));
   CAP_CUDA(cudaEventRecord(e, ps));
   CAP_CUDA(cudaStreamWaitEvent(ctx->copy_out, e, 0));
@@ -330,6 +337,7 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   if (const char* e = getenv("CAPITAL_TF32_MIN_K")) ctx->tf32_min_k = atoll(e);
   if (const char* e = getenv("CAPITAL_FAR_MIN")) ctx->far_min = atoll(e);
   if (const char* e = getenv("CAPITAL_SIDE_MIN")) ctx->side_min = atoll(e);
+  if (const char* e = getenv("CAPITAL_BAND_MIN")) ctx->band_min = atoll(e);
   *out = ctx;
   return CAPITAL_OK;
 }

@@ -12,8 +12,18 @@
 // Two streams.  The reference's recursion is strictly sequential; here the chain that the next diagonal block
 // depends on (base cases, R12, and the part of the trailing update the right child's left subtree reads -- "near")
 // runs on a high-priority stream, while work nobody waits for yet (the rest of the trailing update -- "far" -- and
-// T^T of the inverse combine) is queued on a low-priority stream and joined by events exactly where it is consumed.
-// The latency-bound bottom of the recursion then overlaps with DMMA-bound work instead of idling 140 SMs.
+// T^T of the inverse combine) is queued on low-priority streams and joined by events exactly where it is consumed.
+// The latency-bound bottom of the recursion then overlaps with DMMA-bound work instead of idling 140 SMs.  Deferred work that is
+// wanted sooner must not queue behind work that is wanted later, so the deferred streams are split by when their work is needed:
+// the top-level node's far update (~10 ms, needed by the right half's R12) on the lowest-priority stream, the far updates of every
+// other node (needed within a subtree) on a higher-priority one, and the T^T products (needed as soon as a right child returns)
+// on the highest.
+//
+// Bands.  Two products of a node wait on the chain for a whole child although their leading part depends on half of it only:
+// rows [0, r) of R12 = Rinv11^T A12 read Rinv11[0:r, 0:r], the inverse of the left child's own left child, and columns [0, c) of
+// Rinv12 = -(T^T)^T Rinv22 read Rinv22[0:c, 0:c], that of the right child's left child.  These leading bands are issued from inside
+// the child, on a deferred stream of their own, as soon as that grandchild has returned; they then run beside the base cases of
+// the child's right half, and the chain issues only the rest of the product (same tiles, same k ranges: identical results).
 #include "common.cuh"
 
 namespace {
@@ -31,13 +41,17 @@ constexpr int64_t IN_CHUNK = 2048;  // columns per launch of an R12 product issu
 
 struct Rec {
   capital_ctx* ctx;
-  cudaStream_t M, S;  // critical chain / deferred work
+  cudaStream_t M;     // critical chain
+  cudaStream_t S, D;  // deferred far updates and bands of the top-level node / of every other node (nullptr: one stream)
+  cudaStream_t T;     // T^T products
+  bool bands;         // leading bands of R12 / Rinv12 are issued early
   double *W, *R, *Ri, *RiT;
   int64_t ldw, ldr, ldri, ldrit;
   int64_t bc;
   int split;
   const CholinvHooks* hooks;
   int64_t far_min;  // trailing updates smaller than this are not split
+  int64_t band_min;   // nodes whose left part is smaller than this issue their products whole
   int64_t total;      // size of the top-level block
   bool base_aligned;  // all four buffers 16-byte aligned with even leading dimensions (cluster kernel uses 16-byte accesses)
 };
@@ -63,9 +77,50 @@ capital_status_t new_event(capital_ctx* ctx, cudaEvent_t* e) {
   return CAPITAL_OK;
 }
 
-// o: offset of the node inside the buffers (diagonal position); pending: event the node's first use of data outside
-// its leading sub-block has to wait for (the parent's deferred "far" update), or nullptr.
-capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pending, int depth) {
+// The leading band of one of a node's products, handed to the child whose first half it depends on.
+struct Band {
+  bool r12;          // true: rows [0, edge) of R12 (left child); false: columns [0, edge) of Rinv12 and their rows of RiT21 (right child)
+  int64_t o, s1, s2;  // the node
+  cudaEvent_t wait;   // what the operands wait for besides the chain: the node's `pending` (R12) / its T^T (Rinv12), or nullptr
+  cudaStream_t st;    // the node's deferred far-update stream
+  int64_t edge = 0;   // set when issued
+  cudaEvent_t done = nullptr;
+};
+
+// Issue band b on its stream behind everything the chain has issued so far; `split` is the split point of the child that
+// issues it (its left child has just returned), rounded down to whole 128-wide tiles so that every tile keeps its k range.
+capital_status_t issue_band(Rec& r, Band& b, int64_t split) {
+  capital_ctx* ctx = r.ctx;
+  const int64_t edge = split / 128 * 128;
+  if (edge == 0) return CAPITAL_OK;
+  cudaEvent_t e;
+  CAP_TRY(new_event(ctx, &e));
+  CAP_CUDA(cudaEventRecord(e, r.M));
+  CAP_CUDA(cudaStreamWaitEvent(b.st, e, 0));
+  if (b.wait) CAP_CUDA(cudaStreamWaitEvent(b.st, b.wait, 0));
+  const int64_t o = b.o, s1 = b.s1, s2 = b.s2;
+  const int64_t ldw = r.ldw, ldr = r.ldr, ldri = r.ldri, ldrit = r.ldrit;
+  double* Ri = r.Ri + o * ldri + o;
+  if (b.r12) {
+    // R12[0:edge, :] = Rinv11[0:edge, 0:edge]^T A12[0:edge, :]
+    CAP_TRY(gemm_tn(ctx, b.st, edge, s2, edge, 1.0, Ri, ldri, r.W + (o + s1) * ldw + o, ldw, 0.0, r.R + (o + s1) * ldr + o, ldr,
+                    CAPITAL_GEMM_A_UPPER));
+  } else {
+    // Rinv12[:, 0:edge] = -(T^T)^T Rinv22[0:edge, 0:edge]
+    double* Ri12 = Ri + s1 * ldri;
+    CAP_TRY(gemm_tn(ctx, b.st, s1, edge, edge, -1.0, r.W + o * ldw + o + s1, ldw, Ri12 + s1, ldri, 0.0, Ri12, ldri, CAPITAL_GEMM_B_UPPER));
+    CAP_TRY(transpose_block(ctx, b.st, s1, edge, Ri12, ldri, r.RiT + o * ldrit + o + s1, ldrit, 1.0));
+  }
+  CAP_TRY(new_event(ctx, &b.done));
+  CAP_CUDA(cudaEventRecord(b.done, b.st));
+  b.edge = edge;
+  return CAPITAL_OK;
+}
+
+// o: offset of the node inside the buffers (diagonal position); pending / pending22: events the node's first use of A12 / A22 has to
+// wait for (the two parts of the parent's deferred "far" update, recorded in this order on the deferred stream), or nullptr; up: the
+// parent's band this node issues once its left child has returned, or nullptr.
+capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pending, cudaEvent_t pending22, int depth, Band* up) {
   capital_ctx* ctx = r.ctx;
   double* W = r.W + o * r.ldw + o;
   double* R = r.R + o * r.ldr + o;
@@ -75,7 +130,7 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   const int64_t s1 = choose_split(r, o, n, complete);
   if (s1 == 0) {
     if (r.hooks && r.hooks->need_cols) CAP_TRY(r.hooks->need_cols(r.hooks->user, r.M, o + n));
-    if (pending) CAP_CUDA(cudaStreamWaitEvent(r.M, pending, 0));
+    if (pending22) CAP_CUDA(cudaStreamWaitEvent(r.M, pending22, 0));
     if (n <= LEAF_MAX) CAP_TRY(leaf_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
     else CAP_TRY(basecase_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
     return CAPITAL_OK;
@@ -89,7 +144,11 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   double* Ri22 = Ri + s1 * ldri + s1;
   double* RiT21 = RiT + s1;
 
-  CAP_TRY(rec(r, o, s1, true, nullptr, depth + 1));
+  cudaStream_t F = depth == 0 ? r.S : r.D;  // this node's deferred far updates and bands
+  const bool bands = r.bands && s1 >= r.band_min;
+  Band b12{true, o, s1, s2, pending, F};
+  CAP_TRY(rec(r, o, s1, true, nullptr, nullptr, depth + 1, bands ? &b12 : nullptr));
+  if (up) CAP_TRY(issue_band(r, *up, s1));
   // right spine only (o + n == total size): everything left of column o + s1 is final for R
   if (depth <= 3 && o + n == r.total && r.hooks && r.hooks->left_done) CAP_TRY(r.hooks->left_done(r.hooks->user, r.M, o + s1, depth));
   // "trsm" via the inverse (cholinv.hpp:116-122): R12 = Rinv11^T A12
@@ -106,17 +165,23 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
     }
   } else {
     if (r.hooks && r.hooks->need_cols) CAP_TRY(r.hooks->need_cols(r.hooks->user, r.M, o + n));
-    if (pending) CAP_CUDA(cudaStreamWaitEvent(r.M, pending, 0));  // the parent's deferred update covers W12 and W22
-    CAP_TRY(gemm_tn(ctx, r.M, s1, s2, s1, 1.0, Ri, ldri, W12, ldw, 0.0, R12, ldr, CAPITAL_GEMM_A_UPPER));
+    if (pending) CAP_CUDA(cudaStreamWaitEvent(r.M, pending, 0));  // the first part of the parent's deferred update covers W12
+    // rows [0, e) are the band already issued from inside the left child
+    const int64_t e = b12.edge;
+    CAP_TRY(gemm_tn_off(ctx, r.M, s1 - e, s2, s1, 1.0, Ri + e * ldri, ldri, W12, ldw, 0.0, R12 + e, ldr, CAPITAL_GEMM_A_UPPER, 0, (int)e));
+    if (b12.done) CAP_CUDA(cudaStreamWaitEvent(r.M, b12.done, 0));
   }
-  cudaEvent_t e_r12 = nullptr, e_tt = nullptr, e_far = nullptr;
+  // the trailing update accumulates into W22: the whole of the parent's deferred update has to be in
+  if (pending22) CAP_CUDA(cudaStreamWaitEvent(r.M, pending22, 0));
+  cudaEvent_t e_r12 = nullptr, e_tt = nullptr, e_far12 = nullptr, e_far = nullptr;
   const bool use_side = r.S != nullptr && s1 >= r.ctx->side_min;
   if (use_side) {
     CAP_TRY(new_event(ctx, &e_r12));
     CAP_CUDA(cudaEventRecord(e_r12, r.M));
-    CAP_CUDA(cudaStreamWaitEvent(r.S, e_r12, 0));
+    CAP_CUDA(cudaStreamWaitEvent(F, e_r12, 0));
+    if (complete) CAP_CUDA(cudaStreamWaitEvent(r.T, e_r12, 0));
   }
-  cudaStream_t tS = use_side ? r.S : r.M;
+  cudaStream_t tS = use_side ? r.T : r.M;
   // trailing update (cholinv.hpp:131-134): A22 -= R12^T R12, upper tiles only.
   // near = what the right child's left subtree reads (leading h x h block), far = everything else.
   const int64_t h = choose_split(r, o + s1, s2, true);
@@ -125,17 +190,21 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   if (use_side && h > 0 && s2 >= r.far_min) {
     if (tf) {
       CAP_TRY(gemm_tn_tf32(ctx, r.M, h, h, s1, -1.0, R12, ldr, R12, ldr, 1.0, W22, ldw, CAPITAL_GEMM_C_UPPER, tf));
-      CAP_TRY(gemm_tn_tf32(ctx, r.S, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0, tf));
-      CAP_TRY(gemm_tn_tf32(ctx, r.S, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
+      CAP_TRY(gemm_tn_tf32(ctx, F, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0, tf));
+      CAP_TRY(new_event(ctx, &e_far12));
+      CAP_CUDA(cudaEventRecord(e_far12, F));
+      CAP_TRY(gemm_tn_tf32(ctx, F, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
                            CAPITAL_GEMM_C_UPPER, tf));
     } else {
       CAP_TRY(gemm_tn(ctx, r.M, h, h, s1, -1.0, R12, ldr, R12, ldr, 1.0, W22, ldw, CAPITAL_GEMM_C_UPPER));
-      CAP_TRY(gemm_tn(ctx, r.S, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0));
-      CAP_TRY(gemm_tn(ctx, r.S, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
+      CAP_TRY(gemm_tn(ctx, F, h, s2 - h, s1, -1.0, R12, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw, ldw, 0));
+      CAP_TRY(new_event(ctx, &e_far12));  // the right child's R12 needs only this part
+      CAP_CUDA(cudaEventRecord(e_far12, F));
+      CAP_TRY(gemm_tn(ctx, F, s2 - h, s2 - h, s1, -1.0, R12 + h * ldr, ldr, R12 + h * ldr, ldr, 1.0, W22 + h * ldw + h, ldw,
                       CAPITAL_GEMM_C_UPPER));
     }
     CAP_TRY(new_event(ctx, &e_far));
-    CAP_CUDA(cudaEventRecord(e_far, r.S));
+    CAP_CUDA(cudaEventRecord(e_far, F));
   } else if (tf) {
     CAP_TRY(gemm_tn_tf32(ctx, r.M, s2, s2, s1, -1.0, R12, ldr, R12, ldr, 1.0, W22, ldw, CAPITAL_GEMM_C_UPPER, tf));
   } else {
@@ -143,20 +212,23 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   }
   if (complete) {
     // inverse combine, first half (cholinv.hpp:151): T^T = R12^T Rinv11^T  (B = RiT11, lower triangular) -- nobody needs
-    // it before the right child is done, so it goes to the deferred stream.
+    // it before the right child is done, so it is deferred; on a stream of its own, since on the far updates' stream the T^T of a
+    // small node would wait behind the far update of an ancestor that nobody needs for milliseconds.
     CAP_TRY(gemm_tn(ctx, tS, s2, s1, s1, 1.0, R12, ldr, RiT, ldrit, 0.0, W21, ldw, CAPITAL_GEMM_B_LOWER));
     if (use_side) {
       CAP_TRY(new_event(ctx, &e_tt));
-      CAP_CUDA(cudaEventRecord(e_tt, r.S));
+      CAP_CUDA(cudaEventRecord(e_tt, r.T));
     }
   }
-  CAP_TRY(rec(r, o + s1, s2, true, e_far, depth + 1));
+  const int64_t ct = s2 / 128;  // whole 128-column tiles of the block
+  const bool inv_chunks = depth == 0 && r.hooks && r.hooks->inv_cols && ct >= 32;
+  Band bi{false, o, s1, s2, e_tt, F};
+  CAP_TRY(rec(r, o + s1, s2, true, e_far12, e_far, depth + 1, (bands && complete && !inv_chunks) ? &bi : nullptr));
   if (depth == 0 && r.hooks && r.hooks->right_done) CAP_TRY(r.hooks->right_done(r.hooks->user, r.M));
   if (complete) {
     if (e_tt) CAP_CUDA(cudaStreamWaitEvent(r.M, e_tt, 0));
     //   Rinv12 = -(T^T)^T Rinv22  (B = Ri22, upper triangular)   (cholinv.hpp:152-155)
-    const int64_t ct = s2 / 128;  // whole 128-column tiles of the block
-    if (depth == 0 && r.hooks && r.hooks->inv_cols && ct >= 32) {
+    if (inv_chunks) {
       // last product of the factorization, and the host is waiting for its result: four column chunks (the k extent grows with the
       // column, so the leading half is cheap), each handed to the copy-out stream as soon as it is done; only the D2H of the last,
       // narrow chunk stays exposed.  Chunk edges are multiples of the 128-column tile: every tile computes exactly what it computes
@@ -171,9 +243,13 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
         CAP_TRY(r.hooks->inv_cols(r.hooks->user, r.M, o + s1 + c1));
       }
     } else {
-      CAP_TRY(gemm_tn(ctx, r.M, s1, s2, s2, -1.0, W21, ldw, Ri22, ldri, 0.0, Ri12, ldri, CAPITAL_GEMM_B_UPPER));
+      // columns [0, c) are the band already issued from inside the right child
+      const int64_t c = bi.edge;
+      CAP_TRY(gemm_tn_off(ctx, r.M, s1, s2 - c, s2, -1.0, W21, ldw, Ri22 + c * ldri, ldri, 0.0, Ri12 + c * ldri, ldri, CAPITAL_GEMM_B_UPPER,
+                          (int)c));
     }
-    CAP_TRY(transpose_block(ctx, r.M, s1, s2, Ri12, ldri, RiT21, ldrit, 1.0));
+    CAP_TRY(transpose_block(ctx, r.M, s1, s2 - bi.edge, Ri12 + bi.edge * ldri, ldri, RiT21 + bi.edge, ldrit, 1.0));
+    if (bi.done) CAP_CUDA(cudaStreamWaitEvent(r.M, bi.done, 0));
   }
   return CAPITAL_OK;
 }
@@ -186,6 +262,9 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
   // `st` is the caller-visible stream; the recursion runs on the context's high-priority stream, fenced by events.
   cudaStream_t M = (ctx->hi && allow_side) ? ctx->hi : st;
   cudaStream_t S = (allow_side && ctx->hi && ctx->side && n >= 1024 && !ctx->no_overlap) ? ctx->side : nullptr;
+  cudaStream_t D = S ? ctx->side_deep[0] : nullptr, T = S ? ctx->side_deep[1] : nullptr;
+  // no bands while A is still arriving from the host: there the R12 products follow the arrival of their columns instead
+  const bool bands = S && !(hooks && hooks->need_cols);
   ctx->dep_used = 0;
   cudaEvent_t e_in = nullptr, e_out = nullptr, e_s = nullptr;
   if (M != st) {
@@ -195,16 +274,18 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
     if (S) CAP_CUDA(cudaStreamWaitEvent(S, e_in, 0));
   }
   const bool aligned = ((((uintptr_t)W | (uintptr_t)R | (uintptr_t)Ri | (uintptr_t)RiT) & 15) == 0) && !((ldw | ldr | ldri | ldrit) & 1);
-  Rec r{ctx, M, S, W, R, Ri, RiT, ldw, ldr, ldri, ldrit, bc, split, hooks, ctx->far_min, n, aligned};
+  Rec r{ctx, M, S, D, T, bands, W, R, Ri, RiT, ldw, ldr, ldri, ldrit, bc, split, hooks, ctx->far_min, ctx->band_min, n, aligned};
   // a top-level node the reference treats as its base case (n <= bc, cholinv.hpp:93-104) gets the FULL inverse whatever complete_inv
   // says; the skip of cholinv.hpp:147 only exists where the top node really splits at n >> split
   if (!cholinv_node_splits(n, bc, split)) complete_top = true;
-  CAP_TRY(rec(r, 0, n, complete_top, nullptr, 0));
+  CAP_TRY(rec(r, 0, n, complete_top, nullptr, nullptr, 0, nullptr));
   if (M != st) {
-    if (S) {  // join the deferred stream (all its work has been consumed through events, this is just the fence)
-      CAP_TRY(new_event(ctx, &e_s));
-      CAP_CUDA(cudaEventRecord(e_s, S));
-      CAP_CUDA(cudaStreamWaitEvent(M, e_s, 0));
+    if (S) {  // join the deferred streams (all their work has been consumed through events, this is just the fence)
+      for (cudaStream_t d : {S, D, T}) {
+        CAP_TRY(new_event(ctx, &e_s));
+        CAP_CUDA(cudaEventRecord(e_s, d));
+        CAP_CUDA(cudaStreamWaitEvent(M, e_s, 0));
+      }
     }
     CAP_TRY(new_event(ctx, &e_out));
     CAP_CUDA(cudaEventRecord(e_out, M));

@@ -43,7 +43,8 @@ struct capital_ctx {
   cudaStream_t stream = nullptr;   // main stream (caller's or owned)
   cudaStream_t side = nullptr;     // low-priority stream: deferred ("far") trailing updates, T^T products; lives in a green context
   void* green = nullptr;           // (CUgreenCtx) SM partition of the deferred stream, see make_green_side_stream (api.cu)
-  cudaStream_t side_deep[2] = {nullptr, nullptr};  // deferred streams of recursion depths 1 and 2 (multi-GPU schedule), same partition, rising priority
+  cudaStream_t side_deep[2] = {nullptr, nullptr};  // deferred streams of recursion depths 1 and 2 (multi-GPU schedule; on one GPU they carry
+                                                   // the bands and the T^T products, cholinv_local.cu), same partition, rising priority
   cudaStream_t hi = nullptr;       // high-priority stream: the critical chain of the recursion
   cudaStream_t copy_in = nullptr, copy_out = nullptr;  // H2D / D2H streams of the host-pointer path
   std::vector<cudaEvent_t> dep_pool;  // dependency events (timing disabled), recycled per factor call
@@ -70,6 +71,7 @@ struct capital_ctx {
   bool profiling = false;
   int64_t far_min = 2048;   // trailing updates at least this large are split into near (critical) / far (deferred)   [env CAPITAL_FAR_MIN]
   int64_t side_min = 1024;  // nodes whose left part is at least this large defer T^T to the low-priority stream      [env CAPITAL_SIDE_MIN]
+  int64_t band_min = 4096;  // nodes whose left part is at least this large issue the leading bands of R12 / Rinv12 early [env CAPITAL_BAND_MIN]
   bool no_overlap = false;  // debug / measurement: run the recursion on one stream
   // EXPERIMENTAL, off by default (capital_set_trailing_precision): trailing updates A22 -= R12^T R12 on the TF32 tensor cores
   // (gemm_tf32.cu); 0 = FP64 DMMA, 1 = TF32, 3 = 3 x TF32 with split operands.  Products with k below tf32_min_k stay FP64.
@@ -133,12 +135,12 @@ struct GemmOperands {
   int64_t lda = 0, ldb = 0;
 };
 capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmOperands& ops,
-                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x);
+                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x, int moff = 0);
 capital_status_t gemm_tn(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                          int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags);
 
 capital_status_t gemm_tn_off(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff);
+                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff, int moff = 0);
 capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags);
 capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,

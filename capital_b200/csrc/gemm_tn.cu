@@ -27,6 +27,7 @@ struct GemmParams {
   int rowoffA, rowoffB;  // element offset of the operand's first row inside its (16B-aligned) tensor map
   int flags;
   int noff;    // column index of this window of B / C inside the full operand (column-chunked launches)
+  int moff;    // row index of this window of A / C inside the full operand (row-chunked launches)
   int ksplit;  // gridDim.z chunks of the k range; > 1 => epilogue accumulates with atomics (C pre-initialised, beta ignored)
   int ncls;    // operand classes: the contraction runs over ncls (A_i, B_i) pairs with identical shapes (SUMMA k-slices, summa.hpp:185-193)
   int gm, gn;  // tile grid
@@ -116,12 +117,12 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
   else { tm = lin % gm; tn = lin / gm; }
   if (XMODE == 2 && (tn % p.x.c) != p.x.z) return;  // another layer computes this tile column and stores it here
   const int m0 = tm * BM, n0 = tn * BN;
-  const int n0g = n0 + p.noff;  // column position used by the structure tests
-  if ((flags & CAPITAL_GEMM_C_UPPER) && m0 > n0g + BN - 1) return;  // tile strictly below the diagonal
+  const int m0g = m0 + p.moff, n0g = n0 + p.noff;  // row / column position used by the structure tests
+  if ((flags & CAPITAL_GEMM_C_UPPER) && m0g > n0g + BN - 1) return;  // tile strictly below the diagonal
 
   int kb = 0, ke = p.K;
-  if (flags & CAPITAL_GEMM_A_UPPER) ke = min(ke, m0 + BM);
-  if (flags & CAPITAL_GEMM_A_LOWER) kb = max(kb, m0);
+  if (flags & CAPITAL_GEMM_A_UPPER) ke = min(ke, m0g + BM);
+  if (flags & CAPITAL_GEMM_A_LOWER) kb = max(kb, m0g);
   if (flags & CAPITAL_GEMM_B_UPPER) ke = min(ke, n0g + BN);
   if (flags & CAPITAL_GEMM_B_LOWER) kb = max(kb, n0g);
   kb &= ~(BK - 1);
@@ -242,7 +243,7 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
 #pragma unroll
       for (int i = 0; i < FM; i++) {
         const int row = m0 + wm * WM + i * 8 + g;
-        if (row >= p.M || (upper_only && row > col + p.noff)) continue;
+        if (row >= p.M || (upper_only && row + p.moff > col + p.noff)) continue;
         double v = alpha * acc[i][j][e];
         if (XMODE == 0 && p.ksplit > 1) {
           if (p.kpart) p.kpart[(long long)blockIdx.z * p.kstride + (long long)col * p.ldk + row] = v;
@@ -296,16 +297,17 @@ struct GemmExtra {
 };
 template <class Cfg>
 capital_status_t launch(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, GemmOperands ops, double beta, double* C,
-                        int64_t ldc, int flags, int ksplit, int noff, const GemmXDev* x, const GemmExtra* ex = nullptr) {
+                        int64_t ldc, int flags, int ksplit, int noff, int moff, const GemmXDev* x, const GemmExtra* ex = nullptr) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN;
   GemmParams p{};
   if (ex) { p.Ct = ex->Ct; p.ldct = ex->ldct; p.no_c = ex->no_c; p.kpart = ex->kpart; p.kstride = ex->kstride; p.ldk = ex->ldk; }
-  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc; p.ksplit = ksplit; p.noff = noff;
+  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = beta; p.C = C; p.ldc = ldc; p.ksplit = ksplit;
+  p.noff = noff; p.moff = moff;
   p.ncls = ops.ncls;
   // TMA fetches 16-byte granules: a window that starts on an odd row (8-byte aligned only) cannot be addressed by
   // box coordinates, so it is first copied to an aligned scratch (O(k m) bytes against O(k m n) flops; only odd
   // split points of non-power-of-two sizes ever take this path).
-  const char* sfx = st == ctx->side ? "_side" : "";
+  const char* sfx = st == ctx->side ? "_side" : st == ctx->side_deep[0] ? "_s1" : st == ctx->side_deep[1] ? "_s2" : "";
   int64_t la[GEMM_NCLS_MAX], lb[GEMM_NCLS_MAX];
   for (int c = 0; c < ops.ncls; c++) {
     la[c] = ops.lda; lb[c] = ops.ldb;
@@ -440,15 +442,15 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
   ops.A[0] = A; ops.B[0] = B; ops.lda = lda; ops.ldb = ldb;
   if (ks == 1) {  // one chunk: the tile is stored straight into C
     ctx->counters.kernel_launches--;
-    if (big) return launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, nullptr);
-    return launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, nullptr);
+    if (big) return launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, 0, nullptr);
+    return launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, 1, 0, 0, nullptr);
   }
   GemmExtra ex;
   ex.ldk = round_up(m, 2); ex.kstride = ex.ldk * n;
   CAP_TRY(ctx->workspace("splitk_part", (size_t)ks * ex.kstride * 8, (void**)&ex.kpart));
   const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
-  if (big) CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, nullptr, &ex)));
-  else CAP_TRY((launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, nullptr, &ex)));
+  if (big) CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, 0, nullptr, &ex)));
+  else CAP_TRY((launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C, ldc, flags, (int)ks, 0, 0, nullptr, &ex)));
   ctx->tl_end(st, tli);
   const long long total = m * n;
   const int gr = (int)std::min<long long>((total + 255) / 256, (long long)ctx->num_sms * 4);
@@ -475,8 +477,8 @@ capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
   const bool big = gemm_uses_big(ctx, m, n);
   const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
   capital_status_t rs;
-  if (big) rs = launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, nullptr, &ex);
-  else rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, nullptr, &ex);
+  if (big) rs = launch<CfgBig>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, 0, nullptr, &ex);
+  else rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, 0.0, C ? C : Ct, C ? ldc : m, flags, 1, 0, 0, nullptr, &ex);
   ctx->tl_end(st, tli);
   return rs;
 }
@@ -487,16 +489,16 @@ capital_status_t gemm_tn(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n
 }
 
 capital_status_t gemm_tn_off(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
-                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff) {
+                             int64_t lda, const double* B, int64_t ldb, double beta, double* C, int64_t ldc, int flags, int noff, int moff) {
   GemmOperands ops;
   ops.A[0] = A; ops.B[0] = B; ops.lda = lda; ops.ldb = ldb;
-  return gemm_tn_x(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, noff, nullptr);
+  return gemm_tn_x(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, noff, nullptr, moff);
 }
 
 // General form: `ops.ncls` operand classes, optional fused depth exchange (see GemmXDev).  With an exchange every layer must call
 // this with the same shapes and flags (the tile grid and the tile ownership are functions of them only).
 capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmOperands& ops,
-                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x) {
+                           double beta, double* C, int64_t ldc, int flags, int noff, const GemmXDev* x, int moff) {
   if (m <= 0 || n <= 0) return CAPITAL_OK;
   bool bad = k < 0 || ops.lda < k || ops.ldb < k || ldc < m || (ops.lda & 1) || (ops.ldb & 1) || ops.ncls < 1 || ops.ncls > GEMM_NCLS_MAX;
   for (int c = 0; !bad && c < ops.ncls; c++) bad = !ops.A[c] || !ops.B[c] || ((uintptr_t)ops.A[c] & 7) || ((uintptr_t)ops.B[c] & 7);
@@ -514,6 +516,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
   double f = 2.0 * (double)m * (double)n * (double)k;
   const bool atri = flags & (CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_A_LOWER), btri = flags & (CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_B_LOWER);
   if (atri && btri) f = 2.0 * (double)m * (double)n * (double)k / 3.0;
+  else if (atri && (flags & CAPITAL_GEMM_A_UPPER) && moff > 0 && k >= moff + m) f = (double)m * (double)n * (double)(2 * (int64_t)moff + m + 1);
   else if (atri) f = (double)n * (double)m * (double)(m + 1);
   else if (btri && (flags & CAPITAL_GEMM_B_UPPER) && noff > 0 && k >= noff + n) f = (double)m * (double)n * (double)(2 * (int64_t)noff + n + 1);
   else if (btri) f = (double)m * (double)n * (double)(n + 1);
@@ -529,7 +532,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
       CAP_CUDA(cudaEventRecord(e0, st));
     }
     const int tli = ctx->tl_begin(st, 1, (double)m, (double)n, (double)k * ops.ncls);
-    CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, x)));
+    CAP_TRY((launch<CfgBig>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, moff, x)));
     ctx->tl_end(st, tli);
     if (ctx->profiling) {
       CAP_CUDA(cudaEventRecord(e1, st));
@@ -538,7 +541,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
     return CAPITAL_OK;
   }
   const int tli = ctx->tl_begin(st, 2, (double)m, (double)n, (double)k * ops.ncls);
-  const capital_status_t rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, x);
+  const capital_status_t rs = launch<CfgSmall>(ctx, st, m, n, k, alpha, ops, beta, C, ldc, flags, 1, noff, moff, x);
   ctx->tl_end(st, tli);
   return rs;
 }

@@ -12,6 +12,19 @@ KIND = {1: "gemm128", 2: "gemm64", 3: "basecase", 4: "leaf", 5: "wait", 6: "sign
 SID = {0: "user", 1: "chain", 2: "far0", 3: "far1", 4: "far2", 5: "push0", 6: "push1", 7: "push2", 8: "push3", 9: "pushB", 10: "copyin", 11: "copyout"}
 
 
+def covered(a, b, iv):
+    """length of [a, b] covered by the union of the intervals iv (rows of start, end)"""
+    seg = sorted((max(a, x), min(b, y)) for x, y in iv if y > a and x < b)
+    tot, cs, ce = 0.0, None, None
+    for x, y in seg:
+        if cs is None or x > ce:
+            tot += (ce - cs) if cs is not None else 0.0
+            cs, ce = x, y
+        else:
+            ce = max(ce, y)
+    return tot + ((ce - cs) if cs is not None else 0.0)
+
+
 def main():
     world = int(os.environ.get("WORLD_SIZE", "1")); rank = int(os.environ.get("RANK", "0")); lr = int(os.environ.get("LOCAL_RANK", "0"))
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 16384
@@ -39,10 +52,12 @@ def main():
     if rank == 0:
         t0, t1 = tl[:, 2].min(), tl[:, 3].max()
         print(f"n={n} bcm={bcm} world={world}: {len(tl)} launches, span {t1 - t0:.2f} ms (with event overhead)")
+        # one GPU: far updates (and bands) of the top-level node / of the other nodes, T^T products, packing of finished columns
+        sids = {**SID, **({2: "far-top", 3: "far-low", 4: "tt", 11: "pack"} if world == 1 else {})}
         for sid in sorted(set(tl[:, 0].astype(int))):
             s = tl[tl[:, 0] == sid]
             busy = (s[:, 3] - s[:, 2]).sum()
-            print(f"  stream {SID.get(sid, sid):8s}: {len(s):5d} launches, busy {busy:8.2f} ms, first {s[:, 2].min():7.2f} last {s[:, 3].max():7.2f}")
+            print(f"  stream {sids.get(sid, sid):8s}: {len(s):5d} launches, busy {busy:8.2f} ms, first {s[:, 2].min():7.2f} last {s[:, 3].max():7.2f}")
             for k in sorted(set(s[:, 1].astype(int))):
                 kk = s[s[:, 1] == k]
                 print(f"      {KIND.get(k, k):9s} x{len(kk):5d}  total {(kk[:, 3] - kk[:, 2]).sum():8.2f} ms  max {(kk[:, 3] - kk[:, 2]).max():7.3f}")
@@ -50,6 +65,15 @@ def main():
         ch = ch[np.argsort(ch[:, 2])]
         gaps = ch[1:, 2] - ch[:-1, 3]
         print(f"  chain idle between launches: {gaps[gaps > 0].sum():.2f} ms over {np.sum(gaps > 0.01)} gaps > 10 us; largest {np.sort(gaps)[-5:]}")
+        # how much of the base cases' time has a GEMM of another stream running beside it (first / second half in issue order)
+        bc = ch[ch[:, 1] == 3]
+        other = tl[(tl[:, 0] != 1) & np.isin(tl[:, 1], (1, 2))][:, 2:4]
+        if len(bc):
+            cov = np.array([covered(a, b, other) for a, b in bc[:, 2:4]])
+            d = bc[:, 3] - bc[:, 2]
+            h = len(bc) // 2
+            print(f"  basecase with a deferred GEMM beside it: first half {cov[:h].sum():.2f} of {d[:h].sum():.2f} ms, "
+                  f"second half {cov[h:].sum():.2f} of {d[h:].sum():.2f} ms")
         w = ch[ch[:, 1] == 5]
         if len(w):
             d = w[:, 3] - w[:, 2]
