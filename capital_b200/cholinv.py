@@ -4,6 +4,8 @@
     cholinv.factor(A, args, topo)                                    # cholinv.hpp:6-28  -> args.R, args.Rinv
     R = cholinv.construct_R(args, topo)                              # cholinv.hpp:30-37 -> rect, zero lower
     X = cholinv.solve(args, B, topo)                                 # A X = B from the factors (capital_cholinv_solve_f64)
+    Ainv = cholinv.inverse(args, topo)                               # A^-1 = Rinv Rinv^T (capital_cholinv_inverse_f64)
+    res = cholinv.inverse_residual(A, Ainv, args, topo)              # ||A Ainv - I||_F / ||I||_F (test/inverse/validate.hpp)
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -103,3 +105,45 @@ def solve(args: info, B: torch.Tensor, topo) -> torch.Tensor:
     ctx.check(_lib.lib().capital_cholinv_solve_f64(ctx.handle, n, C.byref(cargs), _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
                                                    args.R.data_ptr(), args.Rinv.data_ptr(), k, Bc.data_ptr(), n, Xc.data_ptr(), n))
     return Xc if B.dim() == 1 else Xc.t().contiguous()
+
+
+def _check_factors(args: info, what: str) -> int:
+    """the local element count of args.R / args.Rinv, or ValueError when `args` holds no factors of args.local_dim"""
+    if args.R is None or args.Rinv is None or args.global_dim <= 0:
+        raise ValueError(f"cholinv.{what}: `args` holds no factors (run cholinv.factor first)")
+    L = args.local_dim
+    count = L * (L + 1) // 2 if args.serialize else L * L
+    if args.R.numel() != count or args.Rinv.numel() != count:
+        raise ValueError(f"cholinv.{what}: args.R / args.Rinv do not hold factors of the local dimension args.local_dim")
+    return count
+
+
+def inverse(args: info, topo) -> torch.Tensor:
+    """A^-1 = Rinv Rinv^T from the factors of a previous `factor(A, args, topo)` (capital_cholinv_inverse_f64).  Returns the local block
+    as a flat float64 tensor with args.Rinv's length and device (pinned on the host): packed upper when args.serialize, else the full,
+    exactly symmetric rect block.  The same bits on every layer of a grid."""
+    count = _check_factors(args, "inverse")
+    dev = args.Rinv.device
+    out = torch.empty(count, dtype=torch.float64, device=dev, pin_memory=dev.type == "cpu")
+    ctx = topo.context()
+    cargs = args._c()
+    ctx.check(_lib.lib().capital_cholinv_inverse_f64(ctx.handle, args.global_dim, C.byref(cargs),
+                                                     _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
+                                                     args.R.data_ptr(), args.Rinv.data_ptr(), out.data_ptr()))
+    return out
+
+
+def inverse_residual(A: matrix, Ainv: torch.Tensor, args: info, topo) -> float:
+    """inverse::validate (test/inverse/validate.hpp:7-34): ||A Ainv - I||_F / ||I||_F, with Ainv as `inverse(args, topo)` returned it."""
+    count = _check_factors(args, "inverse_residual")
+    if not isinstance(A, matrix) or A.num_rows_global != args.global_dim or A.num_columns_global != args.global_dim \
+            or A.num_rows_local != args.local_dim:
+        raise ValueError("cholinv.inverse_residual: A is not the factored matrix's local block")
+    if not isinstance(Ainv, torch.Tensor) or Ainv.dtype != torch.float64 or Ainv.numel() != count or not Ainv.is_contiguous():
+        raise ValueError(f"cholinv.inverse_residual: Ainv must be a contiguous float64 tensor of {count} elements")
+    ctx = topo.context()
+    r = C.c_double()
+    ctx.check(_lib.lib().capital_cholinv_inverse_residual_f64(ctx.handle, A.data.data_ptr(), args.global_dim,
+                                                              _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
+                                                              Ainv.data_ptr(), C.byref(r)))
+    return float(r.value)

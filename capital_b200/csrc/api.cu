@@ -698,6 +698,117 @@ capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const ca
   return CAPITAL_OK;
 }
 
+// Do the byte ranges [a, a + count) and [b, b + count) of two doubles arrays overlap?
+static bool overlaps(const double* a, const double* b, size_t count) {
+  if (!a || !b) return false;
+  const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b, bytes = count * 8;
+  return pa < pb + bytes && pb < pa + bytes;
+}
+
+// A^-1 = Rinv Rinv^T from the factor's outputs: one DMMA product of Rinv^T (lower) with itself, upper tiles only, tile (i, j) running
+// k from max(i, j) -- n^3 / 3 flops.  Where the factor skipped the top-level Rinv12 (complete_inv = 0 and the top node splits at s1),
+// it is rebuilt first with the two products the factor issues for that block (cholinv_local.cu): T^T = R12^T Rinv11^T, then
+// Rinv12 = -(T^T)^T Rinv22, with the same kernel, flags and shapes.  The only buffers are the factor's own workspaces.
+capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                             const double* R_local, const double* Rinv_local, double* Ainv_local) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int64_t Lc = n > 0 ? ceil_div(n, std::max(ctx->grid.d, 1)) : 0;
+  const size_t count = packed ? (size_t)Lc * (Lc + 1) / 2 : (size_t)Lc * Lc;
+  if (!args || !Rinv_local || !Ainv_local || n <= 0 || args->split <= 0 || args->dir != 'U' ||
+      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED) || overlaps(Ainv_local, Rinv_local, count) ||
+      overlaps(Ainv_local, R_local, count)) {
+    ctx->set_error("cholinv::inverse: invalid arguments (Rinv and Ainv non-null, Ainv not overlapping R or Rinv, split > 0 and dir == 'U', "
+                   "packed upper or rect)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  const capital_grid_t& g = ctx->grid;
+  if (g.size > 1) return dist_cholinv_inverse(ctx, n, args, structure, R_local, Rinv_local, Ainv_local);
+  const int64_t L = n, ld = round_up(L, 16);
+  const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
+  const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::inverse: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  double *W, *Ri, *RiT, *dOut;
+  CAP_TRY(ctx->workspace("W", (size_t)ld * L * 8, (void**)&W));
+  CAP_TRY(ctx->workspace("Ri", (size_t)ld * L * 8, (void**)&Ri));
+  CAP_TRY(ctx->workspace("RiT", (size_t)ld * L * 8, (void**)&RiT));
+  // host inputs are staged in the factor's own output buffers; a host output reuses R's once R has been unpacked
+  const double* dRi;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, count, "Rinv_out", &dRi));
+  if (packed) CAP_TRY(unpack_upper(ctx, st, L, dRi, Ri, ld));
+  else CAP_TRY(triu_copy(ctx, st, L, dRi, L, Ri, ld, 0));
+  CAP_TRY(transpose_block(ctx, st, L, L, Ri, ld, RiT, ld, 1.0));  // Rinv^T: lower, exact zeros above the diagonal
+  if (skipped) {
+    const int64_t s1 = L >> args->split, s2 = L - s1;
+    const double* dR;
+    double* Rm;
+    CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Rm));
+    CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+    if (packed) CAP_TRY(unpack_upper(ctx, st, L, dR, Rm, ld));
+    else CAP_TRY(triu_copy(ctx, st, L, dR, L, Rm, ld, 0));
+    CAP_TRY(gemm_tn(ctx, st, s2, s1, s1, 1.0, Rm + s1 * ld, ld, RiT, ld, 0.0, W + s1, ld, CAPITAL_GEMM_B_LOWER));                     // T^T
+    CAP_TRY(gemm_tn(ctx, st, s1, s2, s2, -1.0, W + s1, ld, Ri + s1 * ld + s1, ld, 0.0, Ri + s1 * ld, ld, CAPITAL_GEMM_B_UPPER));  // Rinv12
+    CAP_TRY(transpose_block(ctx, st, s1, s2, Ri + s1 * ld, ld, RiT + s1, ld, 1.0));
+  }
+  // upper tiles of (Rinv^T)^T Rinv^T; the lower-left T^T scratch in W is overwritten or never read
+  CAP_TRY(gemm_tn(ctx, st, L, L, L, 1.0, RiT, ld, RiT, ld, 0.0, W, ld,
+                  CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER));
+  CAP_TRY(cap_stage_out_begin(ctx, Ainv_local, count, "R_out", &dOut));
+  if (packed) CAP_TRY(pack_upper(ctx, st, L, W, ld, dOut, 0));
+  else CAP_TRY(sym_merge(ctx, st, L, W, ld, W, ld, true, dOut, L, 0, 0, 1));  // the lower half is the upper one's mirror, bit for bit
+  if (dOut != Ainv_local) {
+    CAP_TRY(cap_stage_out_end(ctx, Ainv_local, count, dOut));
+    CAP_CUDA(cudaStreamSynchronize(st));
+  }
+  return CAPITAL_OK;
+}
+
+// ||A Ainv - I||_F / ||I||_F (the inverse validator of the reference, test/inverse/validate.hpp:7-34, with the diagonal taken by global
+// index).  A: the full symmetric local block; Ainv in `structure` as capital_cholinv_inverse_f64 wrote it.
+capital_status_t capital_cholinv_inverse_residual_f64(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
+                                                      const double* Ainv_local, double* residual) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!A_local || !Ainv_local || !residual || n <= 0 || (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED)) {
+    ctx->set_error("cholinv::inverse_residual: invalid arguments (A, Ainv, residual non-null, n > 0, packed upper or rect)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  const capital_grid_t& g = ctx->grid;
+  if (g.size > 1) return dist_cholinv_inverse_residual(ctx, A_local, n, structure, Ainv_local, residual);
+  const int64_t L = n, ld = round_up(L, 16);
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  cudaStream_t st = ctx->stream;
+  const double *dA, *dAi;
+  CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
+  CAP_TRY(cap_stage_in(ctx, Ainv_local, packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L, "Ainv_in", &dAi));
+  double *E, *Am, *F, *U;
+  CAP_TRY(ctx->workspace("W", (size_t)ld * L * 8, (void**)&E));
+  CAP_TRY(ctx->workspace("Ri", (size_t)ld * L * 8, (void**)&Am));
+  CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&F));
+  CAP_TRY(copy_block(ctx, st, L, L, dA, L, Am, ld));
+  if (packed) {
+    CAP_TRY(ctx->workspace("RiT", (size_t)ld * L * 8, (void**)&U));
+    CAP_TRY(unpack_upper(ctx, st, L, dAi, U, ld));
+    CAP_TRY(sym_merge(ctx, st, L, U, ld, U, ld, true, F, ld, 0, 0, 1));
+  } else {
+    CAP_TRY(copy_block(ctx, st, L, L, dAi, L, F, ld));
+  }
+  CAP_TRY(gemm_tn(ctx, st, L, L, L, 1.0, Am, ld, F, ld, 0.0, E, ld, 0));  // A^T Ainv = A Ainv
+  CAP_TRY(sub_identity_local(ctx, st, L, E, ld));
+  CAP_CUDA(cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double), st));
+  CAP_TRY(sumsq_block(ctx, st, L, L, E, ld, 0, 0, 0, 1, ctx->d_scalars));
+  double h = 0;
+  CAP_CUDA(cudaMemcpyAsync(&h, ctx->d_scalars, sizeof(double), cudaMemcpyDeviceToHost, st));
+  CAP_CUDA(cudaStreamSynchronize(st));
+  *residual = sqrt(h) / sqrt((double)n);
+  return CAPITAL_OK;
+}
+
 // ---- CholeskyQR2 ------------------------------------------------------------------------------
 capital_status_t capital_cacqr_factor_f64(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, int num_iter,
                                           const capital_cholinv_args_t* ci_args, capital_structure_t rstruct, double* Q_local,

@@ -167,6 +167,10 @@ capital_status_t pack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const 
 capital_status_t unpack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* packed, double* dst, int64_t ldd);
 capital_status_t triu_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst,
                            int64_t ldd, int zero_diag);
+// n x n local block of a symmetric matrix from its computed upper half U: out = U on and above the global diagonal (local (r, c) is
+// global (y + d r, x + d c)), below it the mirror S, read transposed (s_trans: S(c, r), on one GPU S = U) or as it is
+capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* U, int64_t ldu, const double* S, int64_t lds,
+                           bool s_trans, double* out, int64_t ldo, int x, int y, int d);
 capital_status_t gen_symmetric(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,
                                int64_t n_global, int x, int y, int d, int diag_dom);
 capital_status_t gen_random(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,

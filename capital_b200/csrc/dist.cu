@@ -1101,10 +1101,12 @@ capital_status_t dist_cholinv_factor(capital_ctx* ctx, const double* A_local, in
   return cap_check_info(ctx);
 }
 
-// Dry run of cholinv::factor on one rank of a grid: the sequence of synchronisation-relevant operations, 8 int64 per record
-// (kind, stream, a .. f).  No device is touched.
-extern "C" capital_status_t capital_dist_trace_cholinv(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args,
-                                                        int64_t* out, int64_t cap_records, int64_t* n_records) {
+namespace {
+// Dry run of a CholInv-shaped schedule on one rank of a grid: `run(D, arena)` lays out the arena and records the calls; the result is
+// the sequence of synchronisation-relevant operations, 8 int64 per record (kind, stream, a .. f).  No device is touched.
+template <class Run>
+capital_status_t dry_trace(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args, int64_t* out, int64_t cap_records,
+                           int64_t* n_records, Run run) {
   if (!grid || !args || !n_records || args->split <= 0) return CAPITAL_ERR_INVALID;
   capital_ctx fake;
   fake.grid = *grid;
@@ -1120,15 +1122,26 @@ extern "C" capital_status_t capital_dist_trace_cholinv(const capital_grid_t* gri
   if (st == CAPITAL_OK) st = cholinv_shape(D, n, args);
   if (st == CAPITAL_OK) {
     D.trace = &trace;
-    cholinv_layout(D, P.arena);
-    // two consecutive calls: the hazards between factorizations are part of the protocol
-    for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = cholinv_run(D, (const double*)P.arena, args, CAPITAL_UPPERTRI_PACKED, 0);
+    st = run(D, P.arena);
   }
   fake.peer = nullptr;
   if (st != CAPITAL_OK) return st;
   *n_records = (int64_t)trace.size() / TREC;
   if (out) memcpy(out, trace.data(), (size_t)std::min<int64_t>(cap_records, *n_records) * TREC * 8);
   return CAPITAL_OK;
+}
+}  // namespace
+
+// Dry run of cholinv::factor on one rank of a grid (dry_trace).
+extern "C" capital_status_t capital_dist_trace_cholinv(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args,
+                                                        int64_t* out, int64_t cap_records, int64_t* n_records) {
+  return dry_trace(grid, n, args, out, cap_records, n_records, [&](Dist& D, char* arena) {
+    cholinv_layout(D, arena);
+    // two consecutive calls: the hazards between factorizations are part of the protocol
+    capital_status_t st = CAPITAL_OK;
+    for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = cholinv_run(D, (const double*)arena, args, CAPITAL_UPPERTRI_PACKED, 0);
+    return st;
+  });
 }
 
 capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
@@ -1271,6 +1284,190 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
     ctx->counters.d2h_bytes += n * nrhs * 8;
   }
   return cap_check_info(ctx);
+}
+
+// cholinv::inverse on the grid.  A^-1 = Rinv Rinv^T is ONE distributed product of RiT = Rinv^T (lower triangular) with itself, upper
+// tiles only, with the depth reduction in the epilogue as in the factor.  RiT's local block is the transpose of the partner's Rinv
+// block (transpose_dist), pushed to its X and Y consumers.  Where the factor skipped the top-level Rinv12, the two products that
+// invoke issues for that block rebuild it first.  The rect output's lower half is the transpose partner's upper half, merged in
+// (sym_merge).  Every window of a mirror slot is pushed at most once per call.
+namespace {
+struct Inv {
+  DMat Ri, RiT, R, W, C, Ct;
+};
+// one layout for complete and skipped Rinv12 (signature cholinv_inv:L)
+size_t inverse_layout(Dist& D, Inv& v, char* base) {
+  Layout lay(base);
+  const int64_t L = D.L, ld = D.ld;
+  layout_mat(lay, D, v.Ri, ld, L, ROLE_Y | ROLE_T, false);  // T: the partner's RiT; Y: Rinv22 of a rebuilt Rinv12
+  layout_mat(lay, D, v.RiT, ld, L, ROLE_X | ROLE_Y, true);
+  layout_mat(lay, D, v.R, ld, L, ROLE_X, false);  // R12 of a rebuilt Rinv12
+  layout_mat(lay, D, v.W, ld, L, ROLE_X, false);  // T^T of a rebuilt Rinv12 (lower-left block)
+  layout_mat(lay, D, v.C, ld, L, ROLE_T, false);  // upper half of A^-1; T: the partner's lower half of a rect output
+  layout_mat(lay, D, v.Ct, ld, L, 0, false);
+  layout_exchange(lay, D, Q_CHAIN, L, L);
+  return lay.off;
+}
+
+// dRi (and dR when `skipped`): the factor's outputs on the device; dOut: the local output block.  None is touched in a dry run.
+capital_status_t inverse_run(Dist& D, Inv& v, bool skipped, capital_structure_t structure, const double* dRi, const double* dR,
+                             double* dOut) {
+  capital_ctx* ctx = D.ctx;
+  const capital_grid_t& g = D.g;
+  const int64_t L = D.L, ld = D.ld;
+  const int cs = S_CHAIN;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int zdiag = g.y > g.x ? 1 : 0;  // there the local diagonal lies below the global one
+  ctx->comm_used = 0;
+  CAP_TRY(fork_streams(D));
+  if (!D.dry) CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), D.strm(cs)));
+  D.wr(cs, D.me, v.Ri.own, ld, L, L);
+  if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dRi, v.Ri.own, ld));
+  else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dRi, L, v.Ri.own, ld, zdiag));
+  const Win RiT0{&v.RiT, 0, 0};
+  if (!skipped) {
+    CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, 0, 0, L, L, ROLE_T, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, 0, L, L, nullptr, v.RiT.own, ld));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
+  } else {
+    const int64_t s1 = L >> D.split, s2 = L - s1;
+    D.wr(cs, D.me, v.R.own, ld, L, L);
+    if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dR, v.R.own, ld));
+    else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dR, L, v.R.own, ld, zdiag));
+    // the diagonal blocks of Rinv are final: their transposes travel first (RiT12 stays zero: it is never written, nor pushed)
+    CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, 0, 0, s1, s1, ROLE_T, nullptr));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, s1, s1, s2, s2, ROLE_Y | ROLE_T, nullptr));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.R, 0, s1, s1, s2, ROLE_X, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, 0, s1, s1, nullptr, v.RiT.own, ld));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, s1, s1, s2, s2, nullptr, v.RiT.own + s1 * ld + s1, ld));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, 0, 0, s1, s1, ROLE_X | ROLE_Y, nullptr));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, s1, s1, s2, s2, ROLE_X | ROLE_Y, nullptr));
+    // the two products of invoke for the top-level block, with its shapes, flags and chunking:
+    //   T^T = R12^T Rinv11^T (B = RiT11, lower triangular), then Rinv12 = -(T^T)^T Rinv22 (B = Ri22, upper triangular)
+    CAP_TRY(product(D, Q_CHAIN, s2, s1, s1, 1.0, Win{&v.R, 0, s1}, RiT0, 0.0, Win{&v.W, s1, 0}, CAPITAL_GEMM_B_LOWER));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.W, s1, 0, s2, s1, ROLE_X, nullptr));
+    const int nch = (g.size > 1 && D.d > 1 && s2 >= D.chunk_min) ? D.chunks : 1;
+    Token tRi12;
+    CAP_TRY(product_pushed(D, Q_CHAIN, s1, s2, s2, -1.0, Win{&v.W, s1, 0}, Win{&v.Ri, s1, s1}, 0.0, Win{&v.Ri, 0, s1}, CAPITAL_GEMM_B_UPPER,
+                           nullptr, nullptr, ROLE_T, &tRi12, nch));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, s1, s1, s2, &tRi12, v.RiT.own + s1, ld));
+    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, s1, 0, s2, s1, ROLE_X | ROLE_Y, nullptr));
+  }
+  // the upper half of A^-1 = (Rinv^T)^T Rinv^T: tile (i, j) runs k from max(i, j)
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, RiT0, RiT0, 0.0, Win{&v.C, 0, 0},
+                  CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER));
+  if (packed) {
+    D.rd(cs, v.C.own, ld, L, L);
+    DO(D, cs, pack_upper(ctx, D.strm(cs), L, v.C.own, ld, dOut, zdiag));
+  } else {
+    CAP_TRY(push(D, Q_CHAIN, cs, v.C, 0, 0, L, L, ROLE_T, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.C, 0, 0, L, L, nullptr, v.Ct.own, ld));
+    D.rd(cs, v.C.own, ld, L, L);
+    D.rd(cs, v.Ct.own, ld, L, L);
+    DO(D, cs, sym_merge(ctx, D.strm(cs), L, v.C.own, ld, v.Ct.own, ld, false, dOut, L, g.x, g.y, g.d));
+  }
+  return join_streams(D);
+}
+}  // namespace
+
+capital_status_t dist_cholinv_inverse(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                      const double* R_local, const double* Rinv_local, double* Ainv_local) {
+  CAP_TRY(need_comm(ctx));
+  Dist D;
+  CAP_TRY(dist_setup(D, ctx, false));
+  CAP_TRY(cholinv_shape(D, n, args));
+  const int64_t L = D.L;
+  const bool skipped = args->complete_inv == 0 && node_splits(D, L);  // the factor's predicate (cholinv_run)
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::inverse: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  const size_t count = structure == CAPITAL_UPPERTRI_PACKED ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
+  const double *dRi, *dR = nullptr;
+  double* dOut;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, count, "Rinv_out", &dRi));
+  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+  CAP_TRY(cap_stage_out_begin(ctx, Ainv_local, count, "inv_out", &dOut));
+  Inv v;
+  const size_t bytes = inverse_layout(D, v, nullptr);
+  CAP_TRY(arena_prepare(ctx, bytes, "cholinv_inv:" + std::to_string(L)));
+  inverse_layout(D, v, D.P->arena);
+  CAP_TRY(inverse_run(D, v, skipped, structure, dRi, dR, dOut));
+  CAP_TRY(cap_stage_out_end(ctx, Ainv_local, count, dOut));
+  return cap_check_info(ctx);
+}
+
+// Dry run of two consecutive cholinv::inverse calls (rect output: the full schedule, with the partner's half) on one rank of a grid.
+extern "C" capital_status_t capital_dist_trace_cholinv_inverse(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args,
+                                                                int64_t* out, int64_t cap_records, int64_t* n_records) {
+  return dry_trace(grid, n, args, out, cap_records, n_records, [&](Dist& D, char* arena) {
+    Inv v;
+    inverse_layout(D, v, arena);
+    const bool skipped = args->complete_inv == 0 && node_splits(D, D.L);
+    capital_status_t st = CAPITAL_OK;
+    for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = inverse_run(D, v, skipped, CAPITAL_RECT, nullptr, nullptr, nullptr);
+    return st;
+  });
+}
+
+// ||A Ainv - I||_F / ||I||_F on the grid: Ainv is made full (a packed one is merged with its transpose partner's half), one distributed
+// product A^T Ainv = A Ainv, the identity is subtracted on the ranks that hold global diagonal entries (x == y), and the sum of squares
+// is added over all ranks.  Every layer holds the same product, so the sum counts it c times.
+capital_status_t dist_cholinv_inverse_residual(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
+                                               const double* Ainv_local, double* residual) {
+  CAP_TRY(need_comm(ctx));
+  Dist D;
+  CAP_TRY(dist_setup(D, ctx, false));
+  const capital_grid_t& g = D.g;
+  if (n % g.d != 0) { ctx->set_error("distributed cholinv needs d | n"); return CAPITAL_ERR_UNSUPPORTED; }
+  const int64_t L = n / g.d, ld = round_up(L, 16);
+  D.L = L; D.ld = ld; D.split = 1; D.bc_local = L;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const double *dA, *dAi;
+  CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
+  CAP_TRY(cap_stage_in(ctx, Ainv_local, packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L, "Ainv_in", &dAi));
+  DMat Am, F, U, Ut, E;
+  double* ar = nullptr;
+  auto layout = [&](char* base) {
+    Layout lay(base);
+    layout_mat(lay, D, Am, ld, L, ROLE_X, false);
+    layout_mat(lay, D, F, ld, L, ROLE_Y, false);  // the full Ainv
+    layout_mat(lay, D, U, ld, L, ROLE_T, false);  // its packed upper half, unpacked
+    layout_mat(lay, D, Ut, ld, L, 0, false);
+    layout_mat(lay, D, E, ld, L, 0, false);
+    layout_exchange(lay, D, Q_CHAIN, L, L);
+    ar = lay.take((size_t)2 * D.world);
+    return lay.off;
+  };
+  const size_t bytes = layout(nullptr);
+  CAP_TRY(arena_prepare(ctx, bytes, "cholinv_invres:" + std::to_string(L)));
+  layout(D.P->arena);
+  ctx->comm_used = 0;
+  CAP_TRY(fork_streams(D));
+  cudaStream_t st = D.strm(S_CHAIN);
+  CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
+  CAP_TRY(copy_block(ctx, st, L, L, dA, L, Am.own, ld));
+  if (packed) {
+    CAP_TRY(unpack_upper(ctx, st, L, dAi, U.own, ld));
+    CAP_TRY(push(D, Q_CHAIN, S_CHAIN, U, 0, 0, L, L, ROLE_T, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, U, 0, 0, L, L, nullptr, Ut.own, ld));
+    CAP_TRY(sym_merge(ctx, st, L, U.own, ld, Ut.own, ld, false, F.own, ld, g.x, g.y, g.d));
+  } else {
+    CAP_TRY(copy_block(ctx, st, L, L, dAi, L, F.own, ld));
+  }
+  CAP_TRY(push(D, Q_CHAIN, S_CHAIN, Am, 0, 0, L, L, ROLE_X, nullptr));
+  CAP_TRY(push(D, Q_CHAIN, S_CHAIN, F, 0, 0, L, L, ROLE_Y, nullptr));
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, Win{&Am, 0, 0}, Win{&F, 0, 0}, 0.0, Win{&E, 0, 0}, 0));
+  if (g.x == g.y) CAP_TRY(sub_identity_local(ctx, st, L, E.own, ld));  // global (y + d j, x + d i) is diagonal only there
+  CAP_CUDA(cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double), st));
+  CAP_TRY(sumsq_block(ctx, st, L, L, E.own, ld, 0, g.x, g.y, g.d, ctx->d_scalars));
+  CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 1, ar));
+  CAP_TRY(join_streams(D));
+  double h = 0;
+  CAP_CUDA(cudaMemcpyAsync(&h, ctx->d_scalars, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+  CAP_TRY(cap_check_info(ctx));
+  *residual = sqrt(h / g.c) / sqrt((double)n);
+  return CAPITAL_OK;
 }
 
 capital_status_t dist_summa_gemm_tn(capital_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha, const double* A_local,

@@ -11,6 +11,10 @@ capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, 
 capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                     const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
                                     double* X, int64_t ldx);
+capital_status_t dist_cholinv_inverse(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                      const double* R_local, const double* Rinv_local, double* Ainv_local);
+capital_status_t dist_cholinv_inverse_residual(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
+                                               const double* Ainv_local, double* residual);
 capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, int num_iter,
                                    const capital_cholinv_args_t* ci_args, capital_structure_t rstruct, double* Q_local, double* R_local);
 capital_status_t dist_cacqr_apply_qt(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, capital_structure_t rstruct,

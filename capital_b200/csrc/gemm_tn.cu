@@ -515,7 +515,7 @@ capital_status_t gemm_tn_x(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
   // algorithmic flops of this product on THIS device (structure exploited exactly, not tile-rounded)
   double f = 2.0 * (double)m * (double)n * (double)k;
   const bool atri = flags & (CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_A_LOWER), btri = flags & (CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_B_LOWER);
-  if (atri && btri) f = 2.0 * (double)m * (double)n * (double)k / 3.0;
+  if (atri && btri) f = 2.0 * (double)m * (double)n * (double)k / 3.0 * ((flags & CAPITAL_GEMM_C_UPPER) && m == n ? 0.5 : 1.0);
   else if (atri && (flags & CAPITAL_GEMM_A_UPPER) && moff > 0 && k >= moff + m) f = (double)m * (double)n * (double)(2 * (int64_t)moff + m + 1);
   else if (atri) f = (double)n * (double)m * (double)(m + 1);
   else if (btri && (flags & CAPITAL_GEMM_B_UPPER) && noff > 0 && k >= noff + n) f = (double)m * (double)n * (double)(2 * (int64_t)noff + n + 1);

@@ -68,6 +68,30 @@ __global__ void triu_copy_kernel(long long n, const double* src, long long lds, 
   }
 }
 
+// The full local block of a symmetric result of which only the upper half was computed: out(r, c) = U(r, c) where the GLOBAL position
+// (y + d r, x + d c) lies on or above the diagonal, else the mirror source S -- read transposed (S(c, r): U itself on one GPU) or as
+// it is (on a grid: the transpose partner's upper half, already transposed).  One pass over 32 x 32 tiles; a transposed read is
+// staged in shared memory so that it stays coalesced too, and tiles wholly above the diagonal read U only.
+__global__ void sym_merge_kernel(int n, const double* U, long long ldu, const double* S, long long lds, int s_trans, double* out,
+                                 long long ldo, int x, int y, int d) {
+  __shared__ double tile[TP][TP + 1];
+  const int r0 = blockIdx.x * TP, c0 = blockIdx.y * TP;
+  const bool all_upper = y + (long long)d * (r0 + TP - 1) <= x + (long long)d * c0;  // the tile's bottom-left corner is
+  if (s_trans && !all_upper) {
+    for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+      const int r = r0 + j, c = c0 + threadIdx.x;
+      if (r < n && c < n) tile[j][threadIdx.x] = S[(long long)r * lds + c];  // S(c, r)
+    }
+    __syncthreads();
+  }
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    if (r >= n || c >= n) continue;
+    const bool up = y + (long long)d * r <= x + (long long)d * c;
+    out[(long long)c * ldo + r] = up ? U[(long long)c * ldu + r] : (s_trans ? tile[threadIdx.x][j] : S[(long long)c * lds + r]);
+  }
+}
+
 // drand48: X0 = seed<<16 | 0x330E ; X1 = (a X0 + c) mod 2^48 ; value = X1 / 2^48  (structure.hpp:80-85 re-seeds per element)
 __device__ __forceinline__ double drand48_first(unsigned long long seed) {
   const unsigned long long a = 0x5DEECE66DULL, c = 0xBULL, m48 = (1ULL << 48) - 1;
@@ -229,6 +253,14 @@ capital_status_t triu_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const d
                            int zero_diag) {
   if (n <= 0) return CAPITAL_OK;
   triu_copy_kernel<<<(int)(n < ctx->num_sms * 8 ? n : ctx->num_sms * 8), 256, 0, st>>>(n, src, lds, dst, ldd, zero_diag);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* U, int64_t ldu, const double* S, int64_t lds,
+                           bool s_trans, double* out, int64_t ldo, int x, int y, int d) {
+  if (n <= 0) return CAPITAL_OK;
+  dim3 grid((unsigned)ceil_div(n, TP), (unsigned)ceil_div(n, TP)), block(TP, 8);
+  sym_merge_kernel<<<grid, block, 0, st>>>((int)n, U, ldu, S, lds, s_trans ? 1 : 0, out, ldo, x, y, d);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

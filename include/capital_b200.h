@@ -134,6 +134,9 @@ capital_status_t capital_dist_trace_cholinv(const capital_grid_t* grid, int64_t 
  * cross-cube Gram all-reduce).  CAPITAL_ERR_UNSUPPORTED for the other grids. */
 capital_status_t capital_dist_trace_cacqr(const capital_grid_t* grid, int64_t m_global, int64_t n_global, int num_iter,
                                           const capital_cholinv_args_t* ci_args, int64_t* out, int64_t cap_records, int64_t* n_records);
+/* The same for two consecutive capital_cholinv_inverse_f64 calls (rect output) on a square grid. */
+capital_status_t capital_dist_trace_cholinv_inverse(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
+                                                    int64_t* out, int64_t cap_records, int64_t* n_records);
 
 /* ---- generators (device kernels; bit-exact with the reference's drand48-based ones) ---------- */
 /* matrix::distribute_symmetric(x, y, d, d, key, diagonallyDominant) -- structure.hpp:69-103. */
@@ -169,6 +172,25 @@ capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_
 capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
                                            capital_structure_t structure, const double* R_local, const double* Rinv_local,
                                            int64_t nrhs, const double* B, int64_t ldb, double* X, int64_t ldx);
+
+/* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
+ * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
+ * local blocks exactly as the factor wrote them; R_local is read only when the top-level Rinv12 block was skipped (complete_inv = 0
+ * and the top node splits), where that block is rebuilt first with the factor's own two products; it may be NULL otherwise.
+ * Ainv_local: the rank's L x L local block (L = n / d) in `structure`: packed = the upper triangle, column-packed like R (zeros on the
+ * local-diagonal slots of ranks with y > x); rect = the full symmetric block, exactly symmetric (the lower half is the upper half's
+ * mirror, not a second computation).  Identical on the c layers; deterministic.  One DMMA product of n^3 / 3 flops.  Ainv must not
+ * overlap R or Rinv.  Host or device pointers.  One GPU: enqueued on the context stream, synchronous only when Ainv is a host
+ * pointer; the only device memory is the factor's own workspace.  Grid: synchronous; the product uses the peer arena, so the next
+ * factor call re-clears it.  CAPITAL_ERR_UNSUPPORTED when d does not divide n on a grid. */
+capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                             capital_structure_t structure, const double* R_local, const double* Rinv_local,
+                                             double* Ainv_local);
+/* inverse::validate -- test/inverse/validate.hpp:7-34: ||A Ainv - I||_F / ||I||_F over the whole matrix, computed on the device(s),
+ * the diagonal taken by GLOBAL index.  A_local: the full symmetric rect local block (as the generator writes it); Ainv_local: as
+ * capital_cholinv_inverse_f64 wrote it in `structure`. */
+capital_status_t capital_cholinv_inverse_residual_f64(capital_ctx* ctx, const double* A_local, int64_t n_global,
+                                                      capital_structure_t structure, const double* Ainv_local, double* residual);
 
 /* ---- CholeskyQR2 --------------------------------------------------------------------------- */
 /* qr::cacqr<SP,IP>::factor(A, args, topo) -- cacqr.hpp:217-248, on a topo::rect grid c x d x c.  num_iter: 1 = CQR, 2 = CQR2.
