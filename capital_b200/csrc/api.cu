@@ -814,8 +814,8 @@ capital_status_t capital_cacqr_factor_f64(capital_ctx* ctx, const double* A_loca
                                           const capital_cholinv_args_t* ci_args, capital_structure_t rstruct, double* Q_local,
                                           double* R_local) {
   if (!ctx) return CAPITAL_ERR_INVALID;
-  if (!A_local || !Q_local || !R_local || m <= 0 || n <= 0 || num_iter < 1 || num_iter > 2) {
-    ctx->set_error("cacqr::factor: invalid arguments");
+  if (!A_local || !Q_local || !R_local || m <= 0 || n <= 0 || num_iter < 1 || num_iter > 3) {
+    ctx->set_error("cacqr::factor: invalid arguments (A, Q, R non-null, m, n > 0, num_iter 1, 2 or 3)");
     return CAPITAL_ERR_INVALID;
   }
   CAP_CUDA(cudaSetDevice(ctx->device));

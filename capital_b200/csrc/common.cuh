@@ -179,6 +179,14 @@ capital_status_t gen_random(capital_ctx* ctx, cudaStream_t st, double* A, int64_
 capital_status_t sumsq_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, const double* a, int64_t ld,
                              int upper_mode, int x, int y, int d, double* out);
 capital_status_t sub_identity_local(capital_ctx* ctx, cudaStream_t st, int64_t n, double* a, int64_t ld);
+// Gram shift of shifted CholeskyQR3: G(i, i) += coef * trace, the trace summed in a fixed order by one CTA (no atomics), so that
+// every holder of a bit-identical replica of G derives the same shift bits.  gram_shift: the trace of this n x n block.  On a grid
+// the two halves run apart: gram_diag_partial stores the local diagonal's sum to *out, gram_shift_by adds coef * (parts[0] + ...
+// + parts[nparts - 1]), summed in index order, to the local diagonal (parts may have been written by peer GPUs' copy engines).
+capital_status_t gram_shift(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, double coef);
+capital_status_t gram_diag_partial(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* G, int64_t ld, double* out);
+capital_status_t gram_shift_by(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, const double* parts, int nparts,
+                               double coef);
 
 // ---- leaf.cu ----------------------------------------------------------------------------------
 // potrf('U') + trtri('U','N') of one nb x nb block (nb <= LEAF_MAX) in shared memory.

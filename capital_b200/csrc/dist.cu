@@ -1548,12 +1548,16 @@ struct Qr {
 //   QtIn : its transpose (n x lr), read by the apply
 //   QtOut: (optional) transpose of the updated panel = plain store of the apply, for the next sweep
 //   QcOut: the updated panel, column-major = TRANSPOSED store of the apply's epilogue (no separate transpose pass)
-capital_status_t sweep(Qr& q, const double* Qc, int64_t ldqc, const double* QtIn, double* QtOut, double* QcOut, int64_t ldqo, double* Rout) {
+//   shift: (shifted CholeskyQR3, first sweep) G <- G + shift * trace(G) I before the factorization; 0 = none
+capital_status_t sweep(Qr& q, const double* Qc, int64_t ldqc, const double* QtIn, double* QtOut, double* QcOut, int64_t ldqo, double* Rout,
+                       double shift = 0.0) {
   capital_ctx* ctx = q.ctx;
   cudaStream_t st = q.st;
   const int64_t n = q.n, lr = q.lr;
   CAP_TRY(gemm_tn_splitk(ctx, st, n, n, lr, 1.0, Qc, ldqc, Qc, ldqc, q.G, q.ldn, CAPITAL_GEMM_C_UPPER));  // dsyrk 'U','T' (:15)
   if (ctx->grid.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, q.G, q.ldn * n, q.ar));                    // policy.h:82
+  // after the all-reduce G is bit-identical on every rank, so every rank derives the same shift without communicating
+  if (shift > 0.0) CAP_TRY(gram_shift(ctx, st, n, q.G, q.ldn, shift));
   CAP_CUDA(cudaMemsetAsync(q.Ri, 0, (size_t)q.ldn * n * 8, st));
   CAP_CUDA(cudaMemsetAsync(q.RiT, 0, (size_t)q.ldn * n * 8, st));
   CAP_CUDA(cudaMemsetAsync(Rout, 0, (size_t)q.ldn * n * 8, st));
@@ -1572,7 +1576,23 @@ capital_status_t qr1d_arena(capital_ctx* ctx, int64_t count, double** ar) {
 }
 }  // namespace
 
-// ---- CholeskyQR2, 3D grid (c == d) ---------------------------------------------------------------------------------
+// Shifted CholeskyQR3 (Fukaya, Kannan, Nakatsukasa, Yamamoto, Yanagisawa, SIAM J. Sci. Comput. 42(1), 2020): the first sweep factors
+// G + s I with s = 11 (m n + n (n + 1)) u ||A||_2^2, u = 2^-53, bounded with ||A||_2^2 <= ||A||_F^2 = trace(G); s = coef * trace(G).
+// m, n are the global dimensions.
+static double scqr3_shift_coef(int64_t m, int64_t n) {
+  return 11.0 * ((double)m * (double)n + (double)n * (double)(n + 1)) * 0x1p-53;
+}
+// The factorization after the shifted sweep fails only when Q1 = A R1^-1 has a (numerically) dependent column, i.e. A is numerically
+// rank deficient: say so instead of the bare pivot message.
+static capital_status_t scqr3_check_info(capital_ctx* ctx) {
+  const capital_status_t s = cap_check_info(ctx);
+  if (s == CAPITAL_ERR_NOT_SPD)
+    ctx->set_error("cacqr (shifted CholeskyQR3): the sweep after the shifted sweep broke down (" + ctx->err +
+                   "): A is numerically rank deficient");
+  return s;
+}
+
+// ---- CholeskyQR2, 3D grid (c == d) --------------------------------------------------------------------------------
 // qr::cacqr::invoke_3d / sweep_3d (cacqr.hpp:75-120,195-215): Gram matrix by a SUMMA step, cholinv::factor on the n x n Gram
 // matrix over the same grid, Q <- Q R^{-1} by a SUMMA trmm.  Here each of those is the distributed A^T B product of this file:
 //   G    = Q^T Q                      product(X = Q, Y = Q)                   [row Bcast + dgemm + column Reduce + depth Bcast, :92-99]
@@ -1589,6 +1609,13 @@ struct Qr3 {
   Dist* D;
   int64_t ml, nl, ldq, ldn;
   DMat Q, T1, T2, R1, R2, Rt, Rf;
+  // shifted CholeskyQR3 only (num_iter = 3; laid out after everything else, so the other layouts do not change): R3, R2 R1, R3^T
+  // (its own X slots: the partners may still be reading R2^T from Rt's), and the trace partials of the Gram shift, one per diagonal
+  // rank x = y of layer 0 of cube 0 (a 1 x c row)
+  bool shifted = false;
+  double coef = 0.0;
+  DMat R3, R21, Rt3;
+  double* sslots = nullptr;
 };
 size_t qr3_layout(Qr3& q, char* base) {
   Dist& D = *q.D;
@@ -1617,6 +1644,13 @@ size_t qr3_layout(Qr3& q, char* base) {
     const int64_t cols = (int64_t)D.gram_sets * D.ncubes * nl;
     D.gslots = lay.take((size_t)ld * cols);
     if (D.dry && D.trace) D.rec(T_MAT, 0, (const char*)D.gslots - D.P->arena, ld, cols);
+  }
+  if (q.shifted) {
+    layout_mat(lay, D, q.R3, ld, nl, ROLE_T, false);
+    layout_mat(lay, D, q.R21, ld, nl, ROLE_Y, false);
+    layout_mat(lay, D, q.Rt3, ld, nl, ROLE_X, false);
+    q.sslots = lay.take((size_t)D.c);
+    if (D.dry && D.trace) D.rec(T_MAT, 0, (const char*)q.sslots - D.P->arena, 1, D.c);
   }
   return lay.off;
 }
@@ -1666,7 +1700,48 @@ capital_status_t qr3_setup(capital_ctx* ctx, Dist& D, Qr3& q, int64_t m, int64_t
   CAP_TRY(bc_workspace(D));
   return CAPITAL_OK;
 }
-capital_status_t sweep3d(Qr3& q, DMat& Rout) {
+// Gram shift of shifted CholeskyQR3 on the 3D / tunable grid.  After cube_allreduce the local blocks of G are bit-identical on the c
+// layers and in every cube, and the ranks with x = y hold its diagonal.  One replica contributes, layer 0 of cube 0: each of its c
+// diagonal ranks stores its local diagonal's sum into slot x of every diagonal rank of the world (its own slot by the kernel, the
+// others' by the copy engines, then a flag).  Every diagonal rank adds the c slots in x order -- rank order -- so all of them derive the
+// same shift bits.  A later call writes the slots only after the world barrier that opens it (fork_streams), so one set suffices.
+capital_status_t gram_shift_dist(Qr3& q) {
+  Dist& D = *q.D;
+  capital_ctx* ctx = D.ctx;
+  Peer* P = D.P;
+  const capital_grid_t& g = D.g;
+  const unsigned long long e = ++P->sar_epoch;
+  if (g.x != g.y) return CAPITAL_OK;
+  cudaStream_t st = D.strm(S_CHAIN);
+  const int64_t nl = q.nl, ld = q.ldn;
+  if (D.cube == 0 && g.z == 0) {
+    double* mine = q.sslots + g.x;
+    D.rd(S_CHAIN, D.W.own, ld, nl, nl);
+    D.wr(S_CHAIN, D.me, mine, 1, 1, 1);
+    DO(D, S_CHAIN, gram_diag_partial(ctx, st, nl, D.W.own, ld, mine));
+    std::vector<Flag> sig;
+    for (int k = 0; k < D.ncubes; k++)
+      for (int x = 0; x < D.c; x++)
+        for (int z = 0; z < D.c; z++) {
+          const int t = k * g.size + rank_of(g, x, x, z);
+          if (t == D.me) continue;
+          CAP_TRY(D.dma2d(S_CHAIN, t, peer_ptr(P, t, mine), 1, mine, 1, 1, 1));
+          sig.push_back({t, CTRL_SAR + (size_t)D.me, e});
+        }
+    if (!sig.empty()) CAP_TRY(D.signal_flags(S_CHAIN, sig));
+  }
+  std::vector<Flag> w;
+  for (int x = 0; x < D.c; x++) {
+    const int s = rank_of(g, x, x, 0);  // in cube 0, whose world ranks are its cube ranks
+    if (s != D.me) w.push_back({D.me, CTRL_SAR + (size_t)s, e});
+  }
+  if (!w.empty()) CAP_TRY(D.wait_flags(S_CHAIN, w));
+  D.rd(S_CHAIN, q.sslots, 1, 1, D.c);
+  D.wr(S_CHAIN, D.me, D.W.own, ld, nl, nl);
+  DO(D, S_CHAIN, gram_shift_by(ctx, st, nl, D.W.own, ld, q.sslots, D.c, q.coef));
+  return CAPITAL_OK;
+}
+capital_status_t sweep3d(Qr3& q, DMat& Rout, bool shift = false) {
   Dist& D = *q.D;
   capital_ctx* ctx = D.ctx;
   cudaStream_t st = D.strm(S_CHAIN);
@@ -1675,6 +1750,7 @@ capital_status_t sweep3d(Qr3& q, DMat& Rout) {
   CAP_TRY(push(D, Q_CHAIN, S_CHAIN, q.Q, 0, 0, ml, nl, ROLE_X | ROLE_Y | ROLE_T, &tq));
   CAP_TRY(product(D, Q_CHAIN, nl, nl, ml, 1.0, Win{&q.Q, 0, 0}, Win{&q.Q, 0, 0}, 0.0, Win{&D.W, 0, 0}, 0));
   CAP_TRY(cube_allreduce(D, D.W.own, nl, nl));  // tunable grid: the other cubes' rows (no-op on a c == d grid)
+  if (shift) CAP_TRY(gram_shift_dist(q));
   CAP_TRY(invoke(D, 0, nl, true, -1, Token{}, 0));
   D.rd(S_CHAIN, D.R.own, ld, nl, nl);
   D.wr(S_CHAIN, D.me, Rout.own, ld, nl, nl);
@@ -1686,6 +1762,20 @@ capital_status_t sweep3d(Qr3& q, DMat& Rout) {
   CAP_TRY(push(D, Q_CHAIN, S_CHAIN, q.T2, 0, 0, nl, ml, ROLE_T, &t2));
   CAP_TRY(transpose_dist(D, Q_CHAIN, q.T2, 0, 0, nl, ml, &t2, q.Q.own, q.ldq));                                     // Q = T2^T
   return CAPITAL_OK;
+}
+// Rout = Rl Rr = (Rl^T)^T Rr for upper triangular factors (cacqr.hpp:207-209): Rl^T through the transpose partner (Rl has the T role)
+// into Rt (X role), Rr in the Y role
+capital_status_t r_product(Qr3& q, const DMat& Rl, const DMat& Rr, DMat& Rt, DMat& Rout) {
+  Dist& D = *q.D;
+  const int64_t nl = q.nl, ld = q.ldn;
+  Token t2;
+  CAP_TRY(push(D, Q_CHAIN, S_CHAIN, Rl, 0, 0, nl, nl, ROLE_T, &t2));
+  CAP_TRY(transpose_dist(D, Q_CHAIN, Rl, 0, 0, nl, nl, &t2, Rt.own, ld));
+  CAP_TRY(push(D, Q_CHAIN, S_CHAIN, Rt, 0, 0, nl, nl, ROLE_X, nullptr));
+  CAP_TRY(push(D, Q_CHAIN, S_CHAIN, Rr, 0, 0, nl, nl, ROLE_Y, nullptr));
+  D.wr(S_CHAIN, D.me, Rout.own, ld, nl, nl);
+  DO_CUDA(D, S_CHAIN, cudaMemsetAsync(Rout.own, 0, (size_t)ld * nl * 8, D.strm(S_CHAIN)));
+  return product(D, Q_CHAIN, nl, nl, nl, 1.0, Win{&Rt, 0, 0}, Win{&Rr, 0, 0}, 0.0, Win{&Rout, 0, 0}, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER);
 }
 // the schedule of one cacqr::factor call (dry-runnable): dA (device) -> dQ, dR (device)
 capital_status_t cacqr3d_run(Qr3& q, const double* dA, int num_iter, capital_structure_t rstruct, double* dQ, double* dR) {
@@ -1699,19 +1789,18 @@ capital_status_t cacqr3d_run(Qr3& q, const double* dA, int num_iter, capital_str
   DO_CUDA(D, S_CHAIN, cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   D.wr(S_CHAIN, D.me, q.Q.own, q.ldq, ml, nl);
   DO(D, S_CHAIN, copy_block(ctx, st, ml, nl, dA, ml, q.Q.own, q.ldq));
-  CAP_TRY(sweep3d(q, q.R1));
+  CAP_TRY(sweep3d(q, q.R1, num_iter == 3));
   const double* Rfinal = q.R1.own;
-  if (num_iter > 1) {
+  if (num_iter == 3) {
+    // shifted CholeskyQR3: CholeskyQR2 on Q1 = A R1^-1, then R = R3 (R2 R1)
     CAP_TRY(sweep3d(q, q.R2));
-    // R = R2 R1 = (R2^T)^T R1  (cacqr.hpp:207-209)
-    Token t2;
-    CAP_TRY(push(D, Q_CHAIN, S_CHAIN, q.R2, 0, 0, nl, nl, ROLE_T, &t2));
-    CAP_TRY(transpose_dist(D, Q_CHAIN, q.R2, 0, 0, nl, nl, &t2, q.Rt.own, ld));
-    CAP_TRY(push(D, Q_CHAIN, S_CHAIN, q.Rt, 0, 0, nl, nl, ROLE_X, nullptr));
-    CAP_TRY(push(D, Q_CHAIN, S_CHAIN, q.R1, 0, 0, nl, nl, ROLE_Y, nullptr));
-    D.wr(S_CHAIN, D.me, q.Rf.own, ld, nl, nl);
-    DO_CUDA(D, S_CHAIN, cudaMemsetAsync(q.Rf.own, 0, (size_t)ld * nl * 8, st));
-    CAP_TRY(product(D, Q_CHAIN, nl, nl, nl, 1.0, Win{&q.Rt, 0, 0}, Win{&q.R1, 0, 0}, 0.0, Win{&q.Rf, 0, 0}, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER));
+    CAP_TRY(sweep3d(q, q.R3));
+    CAP_TRY(r_product(q, q.R2, q.R1, q.Rt, q.R21));
+    CAP_TRY(r_product(q, q.R3, q.R21, q.Rt3, q.Rf));
+    Rfinal = q.Rf.own;
+  } else if (num_iter > 1) {
+    CAP_TRY(sweep3d(q, q.R2));
+    CAP_TRY(r_product(q, q.R2, q.R1, q.Rt, q.Rf));  // R = R2 R1
     Rfinal = q.Rf.own;
   }
   const int zd = g.y > g.x ? 1 : 0;  // local diagonal is below the global diagonal on those ranks (cube-square coordinates)
@@ -1727,7 +1816,9 @@ capital_status_t cacqr3d_factor(capital_ctx* ctx, const double* A_local, int64_t
   CAP_CUDA(cudaEventRecord(ctx->ev_start, ctx->stream));
   Dist D;
   Qr3 q{};
-  CAP_TRY(qr3_setup(ctx, D, q, m, n, ci_args, "qr3d"));
+  q.shifted = num_iter == 3;
+  q.coef = scqr3_shift_coef(m, n);
+  CAP_TRY(qr3_setup(ctx, D, q, m, n, ci_args, q.shifted ? "qr3d_s" : "qr3d"));  // the shifted layout is larger: its own signature
   const int64_t ml = q.ml, nl = q.nl;
   const double* dA;
   CAP_TRY(cap_stage_in(ctx, A_local, (size_t)ml * nl, "A_in", &dA));
@@ -1739,7 +1830,7 @@ capital_status_t cacqr3d_factor(capital_ctx* ctx, const double* A_local, int64_t
   CAP_TRY(cap_stage_out_end(ctx, Q_local, (size_t)ml * nl, dQ));
   CAP_TRY(cap_stage_out_end(ctx, R_local, r_count, dR));
   CAP_CUDA(cudaEventRecord(ctx->ev_stop, ctx->stream));
-  return cap_check_info(ctx);
+  return num_iter == 3 ? scqr3_check_info(ctx) : cap_check_info(ctx);
 }
 capital_status_t cacqr3d_residual(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, const double* Q_local,
                                   capital_structure_t rstruct, const double* R_local, double* residual, double* orthogonality) {
@@ -1823,7 +1914,7 @@ inline capital_status_t unsupported_grid(capital_ctx* ctx) {
 extern "C" capital_status_t capital_dist_trace_cacqr(const capital_grid_t* grid, int64_t m, int64_t n, int num_iter,
                                                       const capital_cholinv_args_t* ci_args, int64_t* out, int64_t cap_records,
                                                       int64_t* n_records) {
-  if (!grid || !ci_args || !n_records || ci_args->split <= 0 || num_iter < 1 || num_iter > 2) return CAPITAL_ERR_INVALID;
+  if (!grid || !ci_args || !n_records || ci_args->split <= 0 || num_iter < 1 || num_iter > 3) return CAPITAL_ERR_INVALID;
   if (grid->size < 1 || grid->size > PEER_MAX_RANKS) return CAPITAL_ERR_UNSUPPORTED;
   if (!(grid->c > 1 && grid->c == grid->d) && !use_tune(*grid)) return CAPITAL_ERR_UNSUPPORTED;
   capital_ctx fake;
@@ -1838,6 +1929,8 @@ extern "C" capital_status_t capital_dist_trace_cacqr(const capital_grid_t* grid,
   Dist D;
   D.trace = &trace;
   Qr3 q{};
+  q.shifted = num_iter == 3;
+  q.coef = scqr3_shift_coef(m, n);
   capital_status_t st = qr3_setup(&fake, D, q, m, n, ci_args, "trace", true);
   for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++)
     st = cacqr3d_run(q, (const double*)P.arena, num_iter, CAPITAL_UPPERTRI_PACKED, nullptr, nullptr);
@@ -1892,13 +1985,31 @@ capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int6
   double* Qlast = q_in_place ? dQ : q.Q;
   const int64_t ldlast = q_in_place ? lr : q.ldq;
   const double* Rfinal = q.R1;
-  if (num_iter > 1) {
+  if (num_iter == 3) {
+    // shifted CholeskyQR3: shifted sweep, then CholeskyQR2 on Q1 = A R1^-1.  The transposed panels ping-pong Qt -> Qt2 -> Qt, so
+    // every sweep but the last also emits the transpose the next one reads
+    double* R3;
+    CAP_TRY(ctx->workspace("qrR3", (size_t)q.ldn * n * 8, (void**)&R3));
+    CAP_TRY(sweep(q, Qc, ldqc, q.Qt, q.Qt2, q.Q, q.ldq, q.R1, scqr3_shift_coef(m, n)));
+    CAP_TRY(sweep(q, q.Q, q.ldq, q.Qt2, q.Qt, q.Q, q.ldq, q.R2));
+    CAP_TRY(sweep(q, q.Q, q.ldq, q.Qt, nullptr, Qlast, ldlast, R3));
+    // R = R3 (R2 R1), both products in the R2 R1 form below.  R2 R1 goes to the zeroed G (C_UPPER leaves its lower part zero: the
+    // second product reads whole diagonal tiles of its B operand), R3 R21 to R2, free by then
+    CAP_CUDA(cudaMemsetAsync(q.G, 0, (size_t)q.ldn * n * 8, st));
+    CAP_TRY(transpose_block(ctx, st, n, n, q.R2, q.ldn, q.Rt, q.ldn, 1.0));
+    CAP_TRY(gemm_tn(ctx, st, n, n, n, 1.0, q.Rt, q.ldn, q.R1, q.ldn, 0.0, q.G, q.ldn,
+                    CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));
+    CAP_TRY(transpose_block(ctx, st, n, n, R3, q.ldn, q.Rt, q.ldn, 1.0));
+    CAP_TRY(gemm_tn(ctx, st, n, n, n, 1.0, q.Rt, q.ldn, q.G, q.ldn, 0.0, q.R2, q.ldn,
+                    CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));
+    Rfinal = q.R2;
+  } else if (num_iter > 1) {
     CAP_TRY(sweep(q, Qc, ldqc, q.Qt, q.Qt2, q.Q, q.ldq, q.R1));
     CAP_TRY(sweep(q, q.Q, q.ldq, q.Qt2, nullptr, Qlast, ldlast, q.R2));  // (the apply reads Q^T: the panel may be overwritten)
   } else {
     CAP_TRY(sweep(q, Qc, ldqc, q.Qt, nullptr, Qlast, ldlast, q.R1));
   }
-  if (num_iter > 1) {
+  if (num_iter == 2) {
     // R = R2 R1 (dtrmm, cacqr.hpp:185-187) = (R2^T)^T R1 : A = R2^T (lower), B = R1 (upper)
     CAP_TRY(transpose_block(ctx, st, n, n, q.R2, q.ldn, q.Rt, q.ldn, 1.0));
     CAP_TRY(gemm_tn(ctx, st, n, n, n, 1.0, q.Rt, q.ldn, q.R1, q.ldn, 0.0, q.G, q.ldn,
@@ -1911,7 +2022,7 @@ capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int6
   CAP_TRY(cap_stage_out_end(ctx, Q_local, (size_t)lr * n, dQ));
   CAP_TRY(cap_stage_out_end(ctx, R_local, r_count, dR));
   CAP_CUDA(cudaEventRecord(ctx->ev_stop, st));
-  return cap_check_info(ctx);
+  return num_iter == 3 ? scqr3_check_info(ctx) : cap_check_info(ctx);
 }
 
 capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, const double* Q_local,
@@ -1950,7 +2061,10 @@ capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, in
   if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, G, ldn * n, ar));
   CAP_TRY(sub_identity_local(ctx, st, n, G, ldn));
   CAP_TRY(sumsq_block(ctx, st, n, n, G, ldn, 0, 0, 0, 1, ctx->d_scalars + 2));
-  if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 2, ar));  // numerator/denominator of the residual are row-partitioned sums
+  // numerator/denominator of the residual are row-partitioned sums.  Their slots lie past both halves of G's (in the arena's slack):
+  // peer_allreduce_sum alternates halves by epoch parity, and after a factor with an odd number of sweeps (num_iter 1 or 3) the
+  // scalars' half would start inside the half G's all-reduce is still being summed from on a slower rank (DESIGN §6c, §6d)
+  if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 2, ar + (size_t)2 * g.size * ldn * n));
   double h[3];
   CAP_CUDA(cudaMemcpyAsync(h, ctx->d_scalars, 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CAP_TRY(cap_check_info(ctx));

@@ -172,6 +172,41 @@ __global__ void sub_identity_kernel(long long n, double* a, long long ld) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) a[i * ld + i] -= 1.0;
 }
 
+// Shifted CholeskyQR3: the trace of an n x n block in a fixed order -- thread t adds the diagonal entries t, t + SHIFT_T, ... in
+// turn, then a fixed shared-memory tree -- the same bits for the same block on every GPU.  One CTA of SHIFT_T threads.
+constexpr int SHIFT_T = 256;
+__device__ double diag_sum_cta(long long n, const double* a, long long ld) {
+  __shared__ double red[SHIFT_T];
+  double s = 0.0;
+  for (long long i = threadIdx.x; i < n; i += SHIFT_T) s += a[i * ld + i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int h = SHIFT_T / 2; h; h >>= 1) {
+    if (threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+    __syncthreads();
+  }
+  return red[0];
+}
+__global__ void __launch_bounds__(SHIFT_T) gram_shift_kernel(long long n, double* G, long long ld, double coef) {
+  const double s = coef * diag_sum_cta(n, G, ld);  // every diagonal read is behind the tree's barriers
+  for (long long i = threadIdx.x; i < n; i += SHIFT_T) G[i * ld + i] += s;
+}
+__global__ void __launch_bounds__(SHIFT_T) gram_diag_partial_kernel(long long n, const double* G, long long ld, double* out) {
+  const double s = diag_sum_cta(n, G, ld);
+  if (threadIdx.x == 0) *out = s;
+}
+__global__ void __launch_bounds__(SHIFT_T) gram_shift_by_kernel(long long n, double* G, long long ld, const double* parts, int nparts,
+                                                                double coef) {
+  double t = 0.0;
+  for (int k = 0; k < nparts; k++) {  // system-scope loads: the other partials were stored by peer GPUs' copy engines
+    double v;
+    asm volatile("ld.relaxed.sys.global.f64 %0, [%1];" : "=d"(v) : "l"(parts + k) : "memory");
+    t += v;
+  }
+  const double s = coef * t;
+  for (long long i = threadIdx.x; i < n; i += SHIFT_T) G[i * ld + i] += s;
+}
+
 // zero the band |row - col| <= hw of an n x n matrix
 __global__ void zero_band_kernel(long long n, long long hw, double* a, long long ld) {
   const long long w = 2 * hw + 1, total = n * w;
@@ -285,6 +320,24 @@ capital_status_t sumsq_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, in
 }
 capital_status_t sub_identity_local(capital_ctx* ctx, cudaStream_t st, int64_t n, double* a, int64_t ld) {
   sub_identity_kernel<<<grid_for(ctx, n, 256), 256, 0, st>>>(n, a, ld);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t gram_shift(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, double coef) {
+  if (n <= 0) return CAPITAL_OK;
+  gram_shift_kernel<<<1, SHIFT_T, 0, st>>>(n, G, ld, coef);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t gram_diag_partial(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* G, int64_t ld, double* out) {
+  gram_diag_partial_kernel<<<1, SHIFT_T, 0, st>>>(n, G, ld, out);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t gram_shift_by(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, const double* parts, int nparts,
+                               double coef) {
+  if (n <= 0) return CAPITAL_OK;
+  gram_shift_by_kernel<<<1, SHIFT_T, 0, st>>>(n, G, ld, parts, nparts, coef);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

@@ -30,9 +30,10 @@ constexpr size_t CTRL_BAR = CTRL_DONE + PEER_MAX_RANKS * PEER_Q;  // [src]      
 constexpr size_t CTRL_AR = CTRL_BAR + PEER_MAX_RANKS;             // [src]      small all-reduce epochs
 constexpr size_t CTRL_RED = CTRL_AR + PEER_MAX_RANKS;             // [src][q]   "I have added up the partials of product v of class q"
 constexpr size_t CTRL_GAR = CTRL_RED + PEER_MAX_RANKS * PEER_Q;   // [src]      "my Gram partial of cross-cube all-reduce v has landed"
+constexpr size_t CTRL_SAR = CTRL_GAR + PEER_MAX_RANKS;             // [src]      "my trace partial of Gram shift v has landed" (sCQR3)
 constexpr size_t CTRL_WORDS = 512;
 enum { PEER_WAIT_MEMOP = 0, PEER_WAIT_MEMOP_FLUSH = 1, PEER_WAIT_KERNEL = 2 };
-static_assert(CTRL_GAR + PEER_MAX_RANKS <= CTRL_WORDS, "control block too small");
+static_assert(CTRL_SAR + PEER_MAX_RANKS <= CTRL_WORDS, "control block too small");
 
 typedef int (*peer_allgather_fn)(void* user, const void* send, void* recv, int64_t bytes_per_rank);
 
@@ -57,6 +58,7 @@ struct Peer {
   unsigned long long prod_seq[PEER_QC] = {};        // products with a depth exchange issued so far
   unsigned long long bar_epoch = 0, ar_epoch = 0;
   unsigned long long gar_epoch = 0;                 // cross-cube all-reduces of the tunable grid issued so far (dist.cu)
+  unsigned long long sar_epoch = 0;                 // Gram shifts of shifted CholeskyQR3 on the 3D / tunable grids issued so far
   bool can_flush = false;  // the device accepts CU_STREAM_WAIT_VALUE_FLUSH (attribute + self test at init)
   int wait_mode = 2;    // PEER_WAIT_*: how a stream waits for a peer-written flag [env CAPITAL_PEER_WAIT]
   bool memops = true;   // flags through stream memory operations (no SM needed) instead of one-warp kernels [env CAPITAL_PEER_MEMOPS]

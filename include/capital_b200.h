@@ -131,7 +131,8 @@ capital_status_t capital_probe_dmma_f64(capital_ctx* ctx, double* tflops, double
 capital_status_t capital_dist_trace_cholinv(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
                                             int64_t* out, int64_t cap_records, int64_t* n_records);
 /* The same for two consecutive cacqr::factor calls on a rect grid with c == d > 1 (3D) or 1 < c < d (tunable; the trace includes the
- * cross-cube Gram all-reduce).  CAPITAL_ERR_UNSUPPORTED for the other grids. */
+ * cross-cube Gram all-reduce).  num_iter 1, 2 or 3 (3 also records the Gram shift's scalar sum: copies of the trace partials and their
+ * flags, control words CTRL_SAR); other num_iter: CAPITAL_ERR_INVALID.  CAPITAL_ERR_UNSUPPORTED for the other grids. */
 capital_status_t capital_dist_trace_cacqr(const capital_grid_t* grid, int64_t m_global, int64_t n_global, int num_iter,
                                           const capital_cholinv_args_t* ci_args, int64_t* out, int64_t cap_records, int64_t* n_records);
 /* The same for two consecutive capital_cholinv_inverse_f64 calls (rect output) on a square grid. */
@@ -193,7 +194,11 @@ capital_status_t capital_cholinv_inverse_residual_f64(capital_ctx* ctx, const do
                                                       capital_structure_t structure, const double* Ainv_local, double* residual);
 
 /* ---- CholeskyQR2 --------------------------------------------------------------------------- */
-/* qr::cacqr<SP,IP>::factor(A, args, topo) -- cacqr.hpp:217-248, on a topo::rect grid c x d x c.  num_iter: 1 = CQR, 2 = CQR2.
+/* qr::cacqr<SP,IP>::factor(A, args, topo) -- cacqr.hpp:217-248, on a topo::rect grid c x d x c.  num_iter: 1 = CQR, 2 = CQR2,
+ *  3 = shifted CholeskyQR3 (an extension beyond the reference; Fukaya et al., SIAM J. Sci. Comput. 42(1), 2020): the first sweep
+ *  factors G + s I, s = 11 (m n + n (n + 1)) 2^-53 trace(G), then CQR2 runs on its Q; R = R3 R2 R1.  It factors A with condition
+ *  numbers up to about 1e12 (CQR2 breaks down past about 1e8), on every grid below, with the same outputs.  A numerically rank
+ *  deficient A returns CAPITAL_ERR_NOT_SPD (the sweep after the shifted one breaks down).  Other num_iter: CAPITAL_ERR_INVALID.
  *  1D (c == 1, d == size): invoke_1d :172-193, sweep_1d :5-29, Gram allreduce policy.h:78-85.  A_local: (m/d) x n rect, Q_local same
  *    shape; R_local: n x n packed upper (or rect), replicated on every rank.
  *  3D (c == d) and tunable (1 < c < d, c | d, at most 16 ranks; sweep_tune :122-170): A_local and Q_local (m/d) x (n/c);
