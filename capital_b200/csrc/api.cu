@@ -16,6 +16,10 @@ capital_status_t capital_ctx::workspace(const std::string& name, size_t bytes, v
     b.p = nullptr; b.bytes = 0;
     CAP_CUDA(cudaMalloc(&b.p, bytes));
     b.bytes = bytes;
+    if (poison_workspace) {  // NaN in every double (and float): a read of a value nobody wrote shows up in the result
+      CAP_CUDA(cudaMemsetAsync(b.p, 0xFF, bytes, cudaStreamLegacy));
+      CAP_CUDA(cudaStreamSynchronize(cudaStreamLegacy));  // the context's streams are non-blocking: they do not wait for it
+    }
   }
   *out = b.p;
   return CAPITAL_OK;
@@ -338,6 +342,7 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   if (const char* e = getenv("CAPITAL_FAR_MIN")) ctx->far_min = atoll(e);
   if (const char* e = getenv("CAPITAL_SIDE_MIN")) ctx->side_min = atoll(e);
   if (const char* e = getenv("CAPITAL_BAND_MIN")) ctx->band_min = atoll(e);
+  if (const char* e = getenv("CAPITAL_POISON_WORKSPACE")) ctx->poison_workspace = atoi(e) != 0;
   *out = ctx;
   return CAPITAL_OK;
 }

@@ -73,6 +73,7 @@ struct capital_ctx {
   int64_t side_min = 1024;  // nodes whose left part is at least this large defer T^T to the low-priority stream      [env CAPITAL_SIDE_MIN]
   int64_t band_min = 4096;  // nodes whose left part is at least this large issue the leading bands of R12 / Rinv12 early [env CAPITAL_BAND_MIN]
   bool no_overlap = false;  // debug / measurement: run the recursion on one stream
+  bool poison_workspace = false;  // debug / tests: fill every (re)allocated workspace with 0xFF bytes (NaN)  [env CAPITAL_POISON_WORKSPACE=1]
   // EXPERIMENTAL, off by default (capital_set_trailing_precision): trailing updates A22 -= R12^T R12 on the TF32 tensor cores
   // (gemm_tf32.cu); 0 = FP64 DMMA, 1 = TF32, 3 = 3 x TF32 with split operands.  Products with k below tf32_min_k stay FP64.
   int trailing_mode = 0;

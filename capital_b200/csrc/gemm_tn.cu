@@ -133,7 +133,8 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
     const int t0 = min(nk, (int)blockIdx.z * per), t1 = min(nk, t0 + per);
     kb += t0 * BK;
     nk = t1 - t0;
-    if (nk == 0) return;
+    // an empty trailing chunk (ceil(nk / per) < ksplit) runs on with no loads and stores a zero partial: the reduction adds every
+    // chunk's slot, and a slot nobody wrote holds whatever the workspace last held
   }
   const int niter = nk * p.ncls;  // the k tiles of every operand class, one after the other
 
@@ -421,7 +422,8 @@ __global__ void splitk_reduce_kernel(long long rows, long long cols, const doubl
 // Split-K variant for short-and-fat products (the tall-skinny Gram matrix, cacqr.hpp:15): C = alpha A^T B with the k range cut
 // into chunks, one CTA per (tile, chunk); the partial tiles go to a workspace and are added up in chunk order by a second kernel
 // (deterministic: the same bits on every run and on every rank).  128 x 128 tiles when the output has them: 3 upper tiles x 44
-// chunks fill the 132 SMs of an H100 for a 256 x 256 Gram matrix.
+// chunks fill the 132 SMs of an H100 for a 256 x 256 Gram matrix.  tests/test_gpu_gram.py restates the choice of ks and the chunking
+// (splitk_chunks) to pick its shapes: change both together.
 capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A,
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags) {
   if (m <= 0 || n <= 0 || k <= 0) return CAPITAL_OK;
