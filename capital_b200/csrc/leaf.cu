@@ -14,6 +14,7 @@
 // rsqrt per pivot instead of a sqrt and a divide.
 #include "common.cuh"
 #include <cooperative_groups.h>
+#include <cfloat>
 #include <stdlib.h>
 #include <type_traits>
 namespace cg = cooperative_groups;
@@ -262,6 +263,20 @@ __device__ __forceinline__ void warp_potrf_trtri_32(double (&c)[32], double* __r
   // rsqrt(a) and rsqrt(det) are independent and overlap: one rsqrt latency per TWO pivots on the chain.
   //   R(k,k) = a ra          R(k,j)   = A(k,j) ra                       (ra = 1/sqrt(a))
   //   R(k+1,k+1) = det rdet ra         R(k+1,j) = (A(k+1,j) - l ra R(k,j)) sqrt(a) rdet   (rdet = 1/sqrt(det))
+  // a b and l^2 leave the double range long before the matrix does (diagonal entries below ~1e-154 or above ~1e154, or a graded
+  // block whose neighbouring diagonal entries multiply past 2^+-1024).  Pivots never exceed their diagonal entries and fall 2^111
+  // below them only in a matrix that is singular to working precision, so a block whose diagonal lies in [2^-400, 2^400] -- every
+  // block of ordinary scale -- keeps all pairs in range.  Any other block is equilibrated first: S = D^-1 A D^-1 with
+  // D = diag(2^e), diag(S) in [1, 4), exact in powers of two; then R = R(S) D and 1/R(k,k) = 2^-e_k / R_S(k,k).  The vote makes
+  // the branch warp-uniform, and the pivot loop itself is the same for both.
+  double dl = 0.0;  // A(lane, lane)
+  static_for<0, 32>([&](auto ic) { constexpr int i = decltype(ic)::value; if (lane == i) dl = c[i]; });
+  const bool equil = !__all_sync(0xffffffffu, dl >= 0x1p-400 && dl <= 0x1p400);
+  double fl = 1.0;  // 2^-e of this lane's row and column (1 for a non-positive diagonal entry, which is then reported as before)
+  if (equil) {
+    if (dl > 0.0 && dl <= DBL_MAX) fl = ldexp(1.0, -(ilogb(dl) >> 1));
+    static_for<0, 32>([&](auto ic) { constexpr int i = decltype(ic)::value; c[i] = c[i] * shfl_d(fl, i) * fl; });
+  }
   double a = shfl_d(c[0], 0), l = shfl_d(c[0], 1), b = shfl_d(c[1], 1);
   static_for<0, 32, 2>([&](auto kc) {
     constexpr int k = decltype(kc)::value;
@@ -294,6 +309,11 @@ __device__ __forceinline__ void warp_potrf_trtri_32(double (&c)[32], double* __r
       });
     }
   });
+  if (equil) {
+    const double gl = 1.0 / fl;  // 2^e_lane, exact
+    static_for<0, 32>([&](auto ic) { constexpr int i = decltype(ic)::value; c[i] *= gl; });
+    myrs *= fl;
+  }
   if (dbg2 && lane == 0) dbg2[1] = clock64();
 #pragma unroll
   for (int i = 0; i < 32; i++) sRb[lane * TLD + i] = c[i];  // c[i] == 0 below the diagonal by construction (u = 0 for lane < k)
