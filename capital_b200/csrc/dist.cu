@@ -432,6 +432,11 @@ void layout_exchange(Layout& lay, Dist& D, int q, int64_t m, int64_t n) {
   }
 }
 
+// slot set of peer_allreduce_sum over `world` ranks, for sums of up to `cap` doubles
+ArSlots layout_allreduce(Layout& lay, int world, int64_t cap) {
+  return {lay.take((size_t)2 * world * cap), cap};
+}
+
 // ---- push: a finished block goes to everybody who will read it ----------------------------------------------------------
 // Logical event of class q (counted identically on every rank).  As a SOURCE: after the work enqueued so far on `after_sid`, DMA the
 // window into the mirror slot of every rank that consumes from me in one of `roles`, then raise that rank's flag to the event id.
@@ -957,9 +962,12 @@ size_t cholinv_layout(Dist& D, char* base) {
   return lay.off;
 }
 
-// reserve the arena for a layout; a layout the arena has not held before starts from zeros (mirror slots are only ever written
+// lay out the arena: `layout(base)` assigns the layout's pointers relative to `base` and returns its size in bytes.  It is measured,
+// the arena reserved, then laid out.  A layout the arena has not held before starts from zeros (mirror slots are only ever written
 // where a block is pushed; the triangular products read whole diagonal tiles and rely on zeros elsewhere)
-capital_status_t arena_prepare(capital_ctx* ctx, size_t bytes, const std::string& signature) {
+template <class Fn>
+capital_status_t arena_layout(capital_ctx* ctx, const std::string& signature, Fn layout) {
+  const size_t bytes = layout(nullptr);
   CAP_TRY(peer_arena_reserve(ctx, bytes));
   if (ctx->arena_signature != signature) {
     // (every rank changes layout in the same call.)  A peer may still be pushing blocks of the previous layout that nobody waits
@@ -969,7 +977,17 @@ capital_status_t arena_prepare(capital_ctx* ctx, size_t bytes, const std::string
     ctx->arena_signature = signature;
     if (ctx->grid.size > 1) CAP_TRY(peer_barrier(ctx, ctx->stream));  // nobody writes into a peer's arena before that peer has cleared it
   }
+  layout(peer_of(ctx)->arena);
   return CAPITAL_OK;
+}
+
+// an arena that holds one slot set of peer_allreduce_sum and nothing else
+capital_status_t arena_allreduce(capital_ctx* ctx, const std::string& signature, int64_t cap, ArSlots* slots) {
+  return arena_layout(ctx, signature, [&](char* base) {
+    Layout lay(base);
+    *slots = layout_allreduce(lay, ctx->grid.size, cap);
+    return lay.off;
+  });
 }
 
 capital_status_t cholinv_run(Dist& D, const double* A_local, const capital_cholinv_args_t* args, capital_structure_t ostruct,
@@ -1088,9 +1106,8 @@ capital_status_t dist_cholinv_factor(capital_ctx* ctx, const double* A_local, in
   const int64_t L = D.L;
   const size_t out_count = ostruct == CAPITAL_UPPERTRI_PACKED ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
   CAP_CUDA(cudaEventRecord(ctx->ev_start, ctx->stream));
-  const size_t bytes = cholinv_layout(D, nullptr);
-  CAP_TRY(arena_prepare(ctx, bytes, "cholinv:" + std::to_string(L) + ":" + std::to_string(D.bc_local) + ":" + std::to_string(D.split)));
-  cholinv_layout(D, D.P->arena);
+  CAP_TRY(arena_layout(ctx, "cholinv:" + std::to_string(L) + ":" + std::to_string(D.bc_local) + ":" + std::to_string(D.split),
+                       [&](char* base) { return cholinv_layout(D, base); }));
   CAP_TRY(bc_workspace(D));
   CAP_TRY(cap_stage_out_begin(ctx, R_local, out_count, "R_out", &D.dR));
   CAP_TRY(cap_stage_out_begin(ctx, Rinv_local, out_count, "Rinv_out", &D.dRinv));
@@ -1157,20 +1174,17 @@ capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, 
   const double *dA, *dRin;
   CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
   CAP_TRY(cap_stage_in(ctx, R_local, r_count, "R_in", &dRin));
-  // layout: E (= R^T R - A) and R with its operand slots, receive buffers for one L x L product, 2 x size x 2 scalars for the sum
+  // layout: E (= R^T R - A) and R with its operand slots, receive buffers for one L x L product, slots for the sum of 2 scalars
   DMat E, Rr;
-  double* ar = nullptr;
-  auto layout = [&](char* base) {
+  ArSlots ar;
+  CAP_TRY(arena_layout(ctx, "cholres:" + std::to_string(L), [&](char* base) {
     Layout lay(base);
     layout_mat(lay, D, E, ld, L, 0, false);
     layout_mat(lay, D, Rr, ld, L, ROLE_X | ROLE_Y, true);
     layout_exchange(lay, D, Q_CHAIN, L, L);
-    ar = lay.take((size_t)2 * g.size * 2);
+    ar = layout_allreduce(lay, g.size, 2);
     return lay.off;
-  };
-  const size_t bytes = layout(nullptr);
-  CAP_TRY(arena_prepare(ctx, bytes, "cholres:" + std::to_string(L)));
-  layout(D.P->arena);
+  }));
   ctx->comm_used = 0;
   CAP_TRY(fork_streams(D));
   cudaStream_t st = D.strm(S_CHAIN);
@@ -1229,11 +1243,9 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
   CAP_TRY(ctx->workspace("solve_T", (size_t)n * SOLVE_W * 8, (void**)&T));
   CAP_TRY(ctx->workspace("solve_T2", (size_t)n * SOLVE_W * 8, (void**)&T2));
   CAP_TRY(ctx->workspace("solve_S", (size_t)n * SOLVE_W * 8, (void**)&S));
-  // the all-reduce always sums whole n x SOLVE_W panels: its two slot sets then keep the same place from one call to the next
   const int64_t count = n * SOLVE_W;
-  const size_t bytes = (size_t)2 * D.world * count * 8;
-  CAP_TRY(arena_prepare(ctx, bytes, "cholsolve:" + std::to_string(n)));
-  double* slots = (double*)D.P->arena;
+  ArSlots slots;
+  CAP_TRY(arena_allreduce(ctx, "cholsolve:" + std::to_string(n), count, &slots));
   CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   // this layer's share [ca, cb) of the window's columns: equal triangle area per layer, the same cut on every rank
   auto share = [&](int64_t r0, int64_t r1, int64_t c0, int64_t c1, int64_t* ca, int64_t* cb) {
@@ -1389,9 +1401,7 @@ capital_status_t dist_cholinv_inverse(capital_ctx* ctx, int64_t n, const capital
   if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
   CAP_TRY(cap_stage_out_begin(ctx, Ainv_local, count, "inv_out", &dOut));
   Inv v;
-  const size_t bytes = inverse_layout(D, v, nullptr);
-  CAP_TRY(arena_prepare(ctx, bytes, "cholinv_inv:" + std::to_string(L)));
-  inverse_layout(D, v, D.P->arena);
+  CAP_TRY(arena_layout(ctx, "cholinv_inv:" + std::to_string(L), [&](char* base) { return inverse_layout(D, v, base); }));
   CAP_TRY(inverse_run(D, v, skipped, structure, dRi, dR, dOut));
   CAP_TRY(cap_stage_out_end(ctx, Ainv_local, count, dOut));
   return cap_check_info(ctx);
@@ -1427,8 +1437,8 @@ capital_status_t dist_cholinv_inverse_residual(capital_ctx* ctx, const double* A
   CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
   CAP_TRY(cap_stage_in(ctx, Ainv_local, packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L, "Ainv_in", &dAi));
   DMat Am, F, U, Ut, E;
-  double* ar = nullptr;
-  auto layout = [&](char* base) {
+  ArSlots ar;
+  CAP_TRY(arena_layout(ctx, "cholinv_invres:" + std::to_string(L), [&](char* base) {
     Layout lay(base);
     layout_mat(lay, D, Am, ld, L, ROLE_X, false);
     layout_mat(lay, D, F, ld, L, ROLE_Y, false);  // the full Ainv
@@ -1436,12 +1446,9 @@ capital_status_t dist_cholinv_inverse_residual(capital_ctx* ctx, const double* A
     layout_mat(lay, D, Ut, ld, L, 0, false);
     layout_mat(lay, D, E, ld, L, 0, false);
     layout_exchange(lay, D, Q_CHAIN, L, L);
-    ar = lay.take((size_t)2 * D.world);
+    ar = layout_allreduce(lay, D.world, 1);
     return lay.off;
-  };
-  const size_t bytes = layout(nullptr);
-  CAP_TRY(arena_prepare(ctx, bytes, "cholinv_invres:" + std::to_string(L)));
-  layout(D.P->arena);
+  }));
   ctx->comm_used = 0;
   CAP_TRY(fork_streams(D));
   cudaStream_t st = D.strm(S_CHAIN);
@@ -1505,17 +1512,14 @@ capital_status_t dist_summa_gemm_tn(capital_ctx* ctx, int64_t m, int64_t n, int6
   Dist D;
   CAP_TRY(dist_setup(D, ctx, false));
   DMat A, B, C;
-  auto layout = [&](char* base) {
+  CAP_TRY(arena_layout(ctx, "summa:" + std::to_string(ml) + ":" + std::to_string(nl) + ":" + std::to_string(kl), [&](char* base) {
     Layout lay(base);
     layout_mat(lay, D, A, ldk, ml, ROLE_X, false);
     layout_mat(lay, D, B, ldk, nl, ROLE_Y, false);
     layout_mat(lay, D, C, ldm, nl, 0, false);
     layout_exchange(lay, D, Q_CHAIN, ml, nl);
     return lay.off;
-  };
-  const size_t bytes = layout(nullptr);
-  CAP_TRY(arena_prepare(ctx, bytes, "summa:" + std::to_string(ml) + ":" + std::to_string(nl) + ":" + std::to_string(kl)));
-  layout(D.P->arena);
+  }));
   ctx->comm_used = 0;
   CAP_TRY(fork_streams(D));
   cudaStream_t st = D.strm(S_CHAIN);
@@ -1539,7 +1543,8 @@ struct Qr {
   capital_ctx* ctx;
   cudaStream_t st;
   int64_t lr, n, ldq, ldn, ldt;
-  double *Q, *Qt, *Qt2, *G, *R1, *R2, *Ri, *RiT, *Rt, *ar;
+  double *Q, *Qt, *Qt2, *G, *R1, *R2, *Ri, *RiT, *Rt;
+  ArSlots ar;
 };
 
 // sweep_1d (cacqr.hpp:5-29): G = Q^T Q, all-reduce, R = chol(G), Rinv, Q <- Q Rinv.  R lands in `Rout`.  Every layout change is
@@ -1565,14 +1570,10 @@ capital_status_t sweep(Qr& q, const double* Qc, int64_t ldqc, const double* QtIn
   // Q <- Q Rinv (dtrmm Right/Upper/NoTrans, :25): (Q Rinv)^T = Rinv^T Q^T, A = Rinv (upper), B = Q^T
   return gemm_tn_t(ctx, st, n, lr, n, 1.0, q.Ri, q.ldn, QtIn, q.ldt, QtOut, q.ldt, QcOut, ldqo, CAPITAL_GEMM_A_UPPER);
 }
-// small all-reduce scratch of the 1D path: an arena region of 2 * size * count doubles
-capital_status_t qr1d_arena(capital_ctx* ctx, int64_t count, double** ar) {
-  *ar = nullptr;
+// the 1D grid's arena: one slot set for the Gram matrix (ldn n doubles), shared by the factor and the validator.  One GPU reserves none.
+capital_status_t qr1d_slots(capital_ctx* ctx, int64_t ldn, int64_t n, ArSlots* ar) {
   if (ctx->grid.size == 1) return CAPITAL_OK;
-  const size_t bytes = (size_t)2 * ctx->grid.size * count * 8 + 4096;
-  CAP_TRY(arena_prepare(ctx, bytes, "qr1d:" + std::to_string(count)));
-  *ar = (double*)peer_of(ctx)->arena;
-  return CAPITAL_OK;
+  return arena_allreduce(ctx, "qr1d:" + std::to_string(ldn * n), ldn * n, ar);
 }
 }  // namespace
 
@@ -1616,6 +1617,9 @@ struct Qr3 {
   double coef = 0.0;
   DMat R3, R21, Rt3;
   double* sslots = nullptr;
+  // the validator only (laid out last as well): slots for the world sum of its 3 scalars
+  bool validator = false;
+  ArSlots vslots;
 };
 size_t qr3_layout(Qr3& q, char* base) {
   Dist& D = *q.D;
@@ -1652,6 +1656,7 @@ size_t qr3_layout(Qr3& q, char* base) {
     q.sslots = lay.take((size_t)D.c);
     if (D.dry && D.trace) D.rec(T_MAT, 0, (const char*)q.sslots - D.P->arena, 1, D.c);
   }
+  if (q.validator) q.vslots = layout_allreduce(lay, D.world, 3);
   return lay.off;
 }
 // The schedule's grid: the context's (c == d), or this rank's cube of a tunable grid -- cube k = y / c holds the ranks
@@ -1693,9 +1698,8 @@ capital_status_t qr3_setup(capital_ctx* ctx, Dist& D, Qr3& q, int64_t m, int64_t
     if (ctx->arena_signature != std::string(tag)) { CAP_CUDA(cudaMemsetAsync(buf, 0, bytes, ctx->stream)); ctx->arena_signature = tag; }
     qr3_layout(q, buf);
   } else {
-    const size_t bytes = qr3_layout(q, nullptr);
-    CAP_TRY(arena_prepare(ctx, bytes, std::string(tag) + ":" + std::to_string(q.ml) + ":" + std::to_string(q.nl) + ":" + std::to_string(D.bc_local)));
-    qr3_layout(q, D.P->arena);
+    CAP_TRY(arena_layout(ctx, std::string(tag) + ":" + std::to_string(q.ml) + ":" + std::to_string(q.nl) + ":" + std::to_string(D.bc_local),
+                         [&](char* base) { return qr3_layout(q, base); }));
   }
   CAP_TRY(bc_workspace(D));
   return CAPITAL_OK;
@@ -1836,6 +1840,7 @@ capital_status_t cacqr3d_residual(capital_ctx* ctx, const double* A_local, int64
                                   capital_structure_t rstruct, const double* R_local, double* residual, double* orthogonality) {
   Dist D;
   Qr3 q{};
+  q.validator = true;
   capital_cholinv_args_t dummy{1, 1, 0, 'U'};
   CAP_TRY(qr3_setup(ctx, D, q, m, n, &dummy, "qr3dres"));
   const capital_grid_t& g = D.g;
@@ -1846,8 +1851,6 @@ capital_status_t cacqr3d_residual(capital_ctx* ctx, const double* A_local, int64
   CAP_TRY(cap_stage_in(ctx, A_local, (size_t)ml * nl, "A_in", &dA));
   CAP_TRY(cap_stage_in(ctx, Q_local, (size_t)ml * nl, "Q_in", &dQ));
   CAP_TRY(cap_stage_in(ctx, R_local, r_count, "R_in", &dRin));
-  double* ar;
-  CAP_TRY(ctx->workspace("q3ar_local", 64, (void**)&ar));  // placeholder when size == 1
   ctx->comm_used = 0;
   CAP_TRY(fork_streams(D));
   cudaStream_t st = D.strm(S_CHAIN);
@@ -1878,7 +1881,7 @@ capital_status_t cacqr3d_residual(capital_ctx* ctx, const double* A_local, int64
   CAP_TRY(sumsq_block(ctx, st, nl, nl, D.W.own, ld, 0, 0, 0, 1, ctx->d_scalars + 2));
   // world sums: the residual's numerator and denominator are row-partitioned (each replicated on the c layers); Q^T Q - I is
   // replicated on the c layers of all ncubes cubes
-  if (world > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 3, q.Rf.own));
+  if (world > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 3, q.vslots));
   CAP_TRY(join_streams(D));
   double h[3];
   CAP_CUDA(cudaMemcpyAsync(h, ctx->d_scalars, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1970,7 +1973,7 @@ capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int6
   CAP_TRY(ctx->workspace("qrRi", nn, (void**)&q.Ri));
   CAP_TRY(ctx->workspace("qrRiT", nn, (void**)&q.RiT));
   CAP_TRY(ctx->workspace("qrRt", nn, (void**)&q.Rt));
-  CAP_TRY(qr1d_arena(ctx, q.ldn * n, &q.ar));
+  CAP_TRY(qr1d_slots(ctx, q.ldn, n, &q.ar));
   CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   // Q <- A (cacqr.hpp:226): the Gram product reads A where it lies when its leading dimension suits TMA (even, 16-byte aligned
   // base); the apply wants the transpose, made once here -- every later layout change happens inside a GEMM epilogue
@@ -2039,13 +2042,14 @@ capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, in
   CAP_TRY(cap_stage_in(ctx, A_local, (size_t)lr * n, "A_in", &dA));
   CAP_TRY(cap_stage_in(ctx, Q_local, (size_t)lr * n, "Q_in", &dQ));
   CAP_TRY(cap_stage_in(ctx, R_local, r_count, "R_in", &dRin));
-  double *Q, *Qt, *Et, *R, *G, *ar;
+  double *Q, *Qt, *Et, *R, *G;
   CAP_TRY(ctx->workspace("qrQ", (size_t)ldq * n * 8, (void**)&Q));
   CAP_TRY(ctx->workspace("qrQt", (size_t)ldn * lr * 8, (void**)&Qt));
   CAP_TRY(ctx->workspace("qrQt2", (size_t)ldn * lr * 8, (void**)&Et));
   CAP_TRY(ctx->workspace("qrR1", (size_t)ldn * n * 8, (void**)&R));
   CAP_TRY(ctx->workspace("qrG", (size_t)ldn * n * 8, (void**)&G));
-  CAP_TRY(qr1d_arena(ctx, ldn * n, &ar));
+  ArSlots ar;
+  CAP_TRY(qr1d_slots(ctx, ldn, n, &ar));
   CAP_TRY(copy_block(ctx, st, lr, n, dQ, lr, Q, ldq));
   if (rstruct == CAPITAL_UPPERTRI_PACKED) CAP_TRY(unpack_upper(ctx, st, n, dRin, R, ldn));
   else CAP_TRY(triu_copy(ctx, st, n, dRin, n, R, ldn, 0));
@@ -2061,10 +2065,8 @@ capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, in
   if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, G, ldn * n, ar));
   CAP_TRY(sub_identity_local(ctx, st, n, G, ldn));
   CAP_TRY(sumsq_block(ctx, st, n, n, G, ldn, 0, 0, 0, 1, ctx->d_scalars + 2));
-  // numerator/denominator of the residual are row-partitioned sums.  Their slots lie past both halves of G's (in the arena's slack):
-  // peer_allreduce_sum alternates halves by epoch parity, and after a factor with an odd number of sweeps (num_iter 1 or 3) the
-  // scalars' half would start inside the half G's all-reduce is still being summed from on a slower rank (DESIGN §6c, §6d)
-  if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 2, ar + (size_t)2 * g.size * ldn * n));
+  // numerator/denominator of the residual are row-partitioned sums
+  if (g.size > 1) CAP_TRY(peer_allreduce_sum(ctx, st, ctx->d_scalars, 2, ar));
   double h[3];
   CAP_CUDA(cudaMemcpyAsync(h, ctx->d_scalars, 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CAP_TRY(cap_check_info(ctx));
@@ -2088,7 +2090,7 @@ capital_status_t qr_rows_grid(capital_ctx* ctx, const char* what) {
 
 // Y = Q^T B and, when R_local is given, X = R^-1 Y (lstsq).  Each rank applies its rows of Q to its rows of B; on the grid the n x
 // SOLVE_W partials are summed by peer_allreduce_sum in rank order, so Y -- and X, since R is replicated -- is bit-identical on every
-// rank.  Every all-reduce of a call sums whole n x SOLVE_W panels, under the arena signature qrls:n.
+// rank.
 capital_status_t dist_cacqr_apply_qt(capital_ctx* ctx, int64_t m, int64_t n, const double* Q_local, capital_structure_t rstruct,
                                      const double* R_local, int64_t nrhs, const double* B_local, int64_t ldb, double* X, int64_t ldx) {
   const char* what = R_local ? "cacqr::lstsq" : "cacqr::apply_QT";
@@ -2107,12 +2109,12 @@ capital_status_t dist_cacqr_apply_qt(capital_ctx* ctx, int64_t m, int64_t n, con
   double* dX = X;
   if (x_host) CAP_TRY(ctx->workspace("lsq_X", (size_t)ldx * nrhs * 8, (void**)&dX));
   const int64_t count = n * SOLVE_W;
-  double *S = nullptr, *slots = nullptr;
+  double* S = nullptr;
+  ArSlots slots;
   if (grid) {
     CAP_TRY(ctx->workspace("lsq_S", (size_t)count * 8, (void**)&S));
     CAP_CUDA(cudaMemsetAsync(S, 0, (size_t)count * 8, st));  // columns past a narrow last panel are summed too
-    CAP_TRY(arena_prepare(ctx, (size_t)2 * g.size * count * 8, "qrls:" + std::to_string(n)));
-    slots = (double*)peer_of(ctx)->arena;
+    CAP_TRY(arena_allreduce(ctx, "qrls:" + std::to_string(n), count, &slots));
     CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   }
   for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {

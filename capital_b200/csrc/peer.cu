@@ -307,11 +307,15 @@ capital_status_t peer_barrier(capital_ctx* ctx, cudaStream_t st) {
   return peer_wait(ctx, st, w);
 }
 
-capital_status_t peer_allreduce_sum(capital_ctx* ctx, cudaStream_t st, double* buf, int64_t count, double* slots) {
+capital_status_t peer_allreduce_sum(capital_ctx* ctx, cudaStream_t st, double* buf, int64_t count, const ArSlots& slots) {
   Peer* P = peer_of(ctx);
   if (!P || P->size == 1) return CAPITAL_OK;
+  if (count > slots.cap) {
+    ctx->set_error("peer_allreduce_sum: " + std::to_string(count) + " doubles exceed the slot capacity " + std::to_string(slots.cap));
+    return CAPITAL_ERR_INVALID;
+  }
   const unsigned long long e = ++P->ar_epoch;
-  double* half = slots + (e & 1) * (size_t)P->size * count;  // a rank can run at most one all-reduce ahead of a peer: two buffers suffice
+  double* half = slots.base + (e & 1) * (size_t)P->size * slots.cap;
   ArDst dst;
   for (int r = 0; r < P->size; r++) dst.p[r] = peer_ptr(P, r, half) + (size_t)P->rank * count;
   const int gx = (int)(count >= 1 << 16 ? 32 : ceil_div(count, 2048) > 0 ? ceil_div(count, 2048) : 1);

@@ -83,6 +83,13 @@ inline unsigned long long* ctrl_ptr(const Peer* P, int r, size_t word) { return 
 capital_status_t peer_signal(capital_ctx* ctx, cudaStream_t st, const FlagList& fl);  // remote (or local) flag stores, ordered after the stream's earlier work
 capital_status_t peer_wait(capital_ctx* ctx, cudaStream_t st, const FlagList& fl);    // the stream stalls until every LOCAL flag has reached its value
 capital_status_t peer_barrier(capital_ctx* ctx, cudaStream_t st);                     // all ranks: everything enqueued on `st` before has completed everywhere
-// sum of `count` doubles over all ranks, in rank order on every rank (bit-identical results); `slots` = arena region of
-// 2 * size * count doubles
-capital_status_t peer_allreduce_sum(capital_ctx* ctx, cudaStream_t st, double* buf, int64_t count, double* slots);
+// Slot set of the small all-reduce: an arena region of two halves of size * cap doubles (room for `cap` doubles per rank).  All-reduce e
+// scatters into half e & 1, whose place does not depend on the count.  Two halves suffice when a rank's consecutive all-reduces are
+// ordered on its stream or separated by a call's opening barrier: a rank raises flag e only after its sum e - 1, so no rank can scatter
+// e + 1 into a half that someone is still summing e - 1 from.
+struct ArSlots {
+  double* base = nullptr;
+  int64_t cap = 0;
+};
+// sum of `count` <= slots.cap doubles over all ranks, in rank order on every rank (bit-identical results)
+capital_status_t peer_allreduce_sum(capital_ctx* ctx, cudaStream_t st, double* buf, int64_t count, const ArSlots& slots);
