@@ -6,6 +6,9 @@
     X = cholinv.solve(args, B, topo)                                 # A X = B from the factors (capital_cholinv_solve_f64)
     Ainv = cholinv.inverse(args, topo)                               # A^-1 = Rinv Rinv^T (capital_cholinv_inverse_f64)
     res = cholinv.inverse_residual(A, Ainv, args, topo)              # ||A Ainv - I||_F / ||I||_F (test/inverse/validate.hpp)
+    C = cholinv.sygst(A2, args, topo)                                # C = R^-T A2 R^-1 for A2 x = l A x (capital_cholinv_sygst_f64)
+    X = cholinv.apply_Rinv(args, Y, topo)                            # R^-1 Y, the back-transform (capital_cholinv_apply_rinv_f64)
+    W = cholinv.apply_RinvT(args, B, topo)                           # R^-T B, whitening
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -131,6 +134,58 @@ def inverse(args: info, topo) -> torch.Tensor:
                                                      _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
                                                      args.R.data_ptr(), args.Rinv.data_ptr(), out.data_ptr()))
     return out
+
+
+def sygst(A: matrix, args: info, topo) -> torch.Tensor:
+    """A x = lambda B x reduced to C y = lambda y with the factors of a previous `factor(B, args, topo)` (capital_cholinv_sygst_f64,
+    LAPACK dsygst itype 1): C = R^-T A R^-1, and x = apply_Rinv(args, y, topo).  A: the symmetric matrix, a `matrix` shaped like the
+    factored B; only its global lower triangle (diagonal included) is read.  Returns the local block of C like `inverse` does: a flat
+    float64 tensor with args.Rinv's length and device (pinned on the host), packed upper when args.serialize, else the full, exactly
+    symmetric rect block.  The same bits on every layer of a grid."""
+    count = _check_factors(args, "sygst")
+    if not isinstance(A, matrix) or A.num_rows_global != args.global_dim or A.num_columns_global != args.global_dim \
+            or A.num_rows_local != args.local_dim or A.num_columns_local != args.local_dim:
+        raise ValueError("cholinv.sygst: A must be a matrix shaped like the factored one")
+    if A.data.dtype != torch.float64 or A.data.numel() != args.local_dim * args.local_dim or not A.data.is_contiguous():
+        raise ValueError("cholinv.sygst: A must hold a contiguous float64 local block")
+    dev = args.Rinv.device
+    out = torch.empty(count, dtype=torch.float64, device=dev, pin_memory=dev.type == "cpu")
+    ctx = topo.context()
+    cargs = args._c()
+    ctx.check(_lib.lib().capital_cholinv_sygst_f64(ctx.handle, args.global_dim, C.byref(cargs),
+                                                   _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
+                                                   args.R.data_ptr(), args.Rinv.data_ptr(), A.data.data_ptr(), out.data_ptr()))
+    return out
+
+
+def _apply_rinv(args: info, B: torch.Tensor, topo, trans: int, what: str) -> torch.Tensor:
+    _check_factors(args, what)
+    if not isinstance(B, torch.Tensor) or B.dtype != torch.float64:
+        raise ValueError(f"cholinv.{what}: B must be a float64 tensor")
+    if B.dim() not in (1, 2) or B.shape[0] != args.global_dim or B.numel() == 0:
+        raise ValueError(f"cholinv.{what}: B must have shape ({args.global_dim},) or ({args.global_dim}, k), got {tuple(B.shape)}")
+    n = args.global_dim
+    k = 1 if B.dim() == 1 else B.shape[1]
+    Bc = B.contiguous() if B.dim() == 1 else B.t().contiguous()  # column-major n x k, ld n
+    Xc = torch.empty_like(Bc)
+    ctx = topo.context()
+    cargs = args._c()
+    ctx.check(_lib.lib().capital_cholinv_apply_rinv_f64(ctx.handle, n, C.byref(cargs), _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
+                                                        args.R.data_ptr(), args.Rinv.data_ptr(), trans, k, Bc.data_ptr(), n,
+                                                        Xc.data_ptr(), n))
+    return Xc if B.dim() == 1 else Xc.t().contiguous()
+
+
+def apply_Rinv(args: info, B: torch.Tensor, topo) -> torch.Tensor:
+    """X = R^-1 B from the factors of a previous `factor` (capital_cholinv_apply_rinv_f64, trans = 0): the back-transform x = R^-1 y of
+    `sygst`.  B as for `solve`; returns X with B's shape and device, bit-identical on every rank."""
+    return _apply_rinv(args, B, topo, 0, "apply_Rinv")
+
+
+def apply_RinvT(args: info, B: torch.Tensor, topo) -> torch.Tensor:
+    """X = R^-T B (capital_cholinv_apply_rinv_f64, trans = 1): whitening.  apply_Rinv(args, apply_RinvT(args, B)) is solve(args, B),
+    bit for bit."""
+    return _apply_rinv(args, B, topo, 1, "apply_RinvT")
 
 
 def inverse_residual(A: matrix, Ainv: torch.Tensor, args: info, topo) -> float:

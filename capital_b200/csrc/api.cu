@@ -641,26 +641,28 @@ capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_
   return CAPITAL_OK;
 }
 
-// A X = B from the factor's outputs.  Rinv complete: X = Rinv (Rinv^T B), two passes over the triangle per panel.  Top-level Rinv12
-// skipped (complete_inv = 0 and the top node splits at s1): the block formula with R12 (the reference's cacqr::solve, cacqr.hpp:44-73)
-//   Y1 = Rinv11^T B1,  Y2 = Rinv22^T (B2 - R12^T Y1),  X2 = Rinv22 Y2,  X1 = Rinv11 (Y1 - R12 X2).
-capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+// A X = B from the factor's outputs (mode SOLVE_FULL), or one of its two halves alone (SOLVE_RINVT: X = Rinv^T B, SOLVE_RINV: X = Rinv B).
+// Rinv complete: X = Rinv (Rinv^T B), two passes over the triangle per panel.  Top-level Rinv12 skipped (complete_inv = 0 and the top
+// node splits at s1): the block formula with R12 (the reference's cacqr::solve, cacqr.hpp:44-73)
+//   Y1 = Rinv11^T B1,  Y2 = Rinv22^T (B2 - R12^T Y1),  X2 = Rinv22 Y2,  X1 = Rinv11 (Y1 - R12 X2),
+// whose first three steps are Y = R^-T B and whose last three are X = R^-1 Y.  A half alone runs exactly the solve's steps of that half,
+// through the same panel intermediate T, so applying both halves in turn gives the solve's bits.
+static capital_status_t cholinv_solve_mode(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                            const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
-                                           double* X, int64_t ldx) {
-  if (!ctx) return CAPITAL_ERR_INVALID;
+                                           double* X, int64_t ldx, int mode, const char* what) {
   if (!args || !Rinv_local || !B || !X || n <= 0 || nrhs < 1 || ldb < n || ldx < n || args->split <= 0 || args->dir != 'U' ||
       (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED)) {
-    ctx->set_error("cholinv::solve: invalid arguments (Rinv, B, X non-null, nrhs >= 1, ldb, ldx >= n, split > 0 and dir == 'U')");
+    ctx->set_error(std::string("cholinv::") + what + ": invalid arguments (Rinv, B, X non-null, nrhs >= 1, ldb, ldx >= n, split > 0 and dir == 'U')");
     return CAPITAL_ERR_INVALID;
   }
   CAP_CUDA(cudaSetDevice(ctx->device));
   const capital_grid_t& g = ctx->grid;
-  if (g.size > 1) return dist_cholinv_solve(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx);
+  if (g.size > 1) return dist_cholinv_solve(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx, mode);
   const int64_t L = n;
   const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
   const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
   if (skipped && !R_local) {
-    ctx->set_error("cholinv::solve: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    ctx->set_error(std::string("cholinv::") + what + ": the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
     return CAPITAL_ERR_INVALID;
   }
   const int64_t s1 = L >> args->split;
@@ -678,22 +680,30 @@ capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const ca
   double *T, *T2;  // panel intermediates, L x SOLVE_W
   CAP_TRY(ctx->workspace("solve_T", (size_t)L * SOLVE_W * 8, (void**)&T));
   CAP_TRY(ctx->workspace("solve_T2", (size_t)L * SOLVE_W * 8, (void**)&T2));
+  // first half: T = R^-T Bp
+  auto half_t = [&](const double* Bp, int64_t w) -> capital_status_t {
+    //                 U    ldu  trans r0  r1  c0  c1  nrhs alpha P  pinc ldp   beta Cin     ldcin C   cinc ldc
+    if (!skipped) return tri_apply(ctx, st, {dRi, ldu, true, 0, L, 0, L, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L});  // Y = Rinv^T B
+    CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, 0, s1, 0, s1, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L}));   // T1 = Y1
+    CAP_TRY(tri_apply(ctx, st, {dR, ldu, true, 0, s1, s1, L, w, -1.0, T, 1, L, 1.0, Bp, ldb, T2, 1, L}));       // T2_2 = B2 - R12^T Y1
+    return tri_apply(ctx, st, {dRi, ldu, true, s1, L, s1, L, w, 1.0, T2, 1, L, 0.0, nullptr, 0, T, 1, L});      // T2 = Y2
+  };
+  // second half: Xp = R^-1 T
+  auto half_n = [&](double* Xp, int64_t w) -> capital_status_t {
+    if (!skipped) return tri_apply(ctx, st, {dRi, ldu, false, 0, L, 0, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx});  // X = Rinv Y
+    CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, s1, L, s1, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx})); // X2
+    CAP_TRY(tri_apply(ctx, st, {dR, ldu, false, 0, s1, s1, L, w, -1.0, Xp, 1, ldx, 1.0, T, L, T2, 1, L}));      // T2_1 = Y1 - R12 X2
+    return tri_apply(ctx, st, {dRi, ldu, false, 0, s1, 0, s1, w, 1.0, T2, 1, L, 0.0, nullptr, 0, Xp, 1, ldx});  // X1
+  };
+  // a half alone goes through T as well (B is copied in, or the result copied out), so X may alias B
   for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
     const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
     const double* Bp = dB + p0 * ldb;
     double* Xp = dX + p0 * ldx;
-    //                 U    ldu  trans r0  r1  c0  c1  nrhs alpha P  pinc ldp   beta Cin     ldcin C   cinc ldc
-    if (!skipped) {
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, 0, L, 0, L, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L}));    // Y = Rinv^T B
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, 0, L, 0, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx}));  // X = Rinv Y
-    } else {
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, 0, s1, 0, s1, w, 1.0, Bp, 1, ldb, 0.0, nullptr, 0, T, 1, L}));   // T1 = Y1
-      CAP_TRY(tri_apply(ctx, st, {dR, ldu, true, 0, s1, s1, L, w, -1.0, T, 1, L, 1.0, Bp, ldb, T2, 1, L}));       // T2_2 = B2 - R12^T Y1
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, true, s1, L, s1, L, w, 1.0, T2, 1, L, 0.0, nullptr, 0, T, 1, L}));    // T2 = Y2
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, s1, L, s1, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx})); // X2
-      CAP_TRY(tri_apply(ctx, st, {dR, ldu, false, 0, s1, s1, L, w, -1.0, Xp, 1, ldx, 1.0, T, L, T2, 1, L}));      // T2_1 = Y1 - R12 X2
-      CAP_TRY(tri_apply(ctx, st, {dRi, ldu, false, 0, s1, 0, s1, w, 1.0, T2, 1, L, 0.0, nullptr, 0, Xp, 1, ldx})); // X1
-    }
+    if (mode != SOLVE_RINV) CAP_TRY(half_t(Bp, w));
+    else CAP_TRY(panel_add(ctx, st, L, w, Bp, ldb, nullptr, 0, T, L));
+    if (mode != SOLVE_RINVT) CAP_TRY(half_n(Xp, w));
+    else CAP_TRY(panel_add(ctx, st, L, w, T, L, nullptr, 0, Xp, ldx));
   }
   if (x_host) {  // only the n rows of each column travel: the caller's rows n .. ldx stay untouched
     CAP_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * 8, dX, (size_t)ldx * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
@@ -703,11 +713,49 @@ capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const ca
   return CAPITAL_OK;
 }
 
-// Do the byte ranges [a, a + count) and [b, b + count) of two doubles arrays overlap?
-static bool overlaps(const double* a, const double* b, size_t count) {
+capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                           const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
+                                           double* X, int64_t ldx) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  return cholinv_solve_mode(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx, SOLVE_FULL, "solve");
+}
+
+// X = R^-1 B (trans = 0: the back-transform of sygst) or X = R^-T B (trans = 1: whitening), each one half of the solve.
+capital_status_t capital_cholinv_apply_rinv_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                                const double* R_local, const double* Rinv_local, int trans, int64_t nrhs, const double* B,
+                                                int64_t ldb, double* X, int64_t ldx) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (trans != 0 && trans != 1) {
+    ctx->set_error("cholinv::apply_rinv: trans must be 0 (X = R^-1 B) or 1 (X = R^-T B)");
+    return CAPITAL_ERR_INVALID;
+  }
+  return cholinv_solve_mode(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx, trans ? SOLVE_RINVT : SOLVE_RINV,
+                            "apply_rinv");
+}
+
+// Do the byte ranges of a[0, na) and b[0, nb), two arrays of doubles, overlap?
+static bool overlaps(const double* a, size_t na, const double* b, size_t nb) {
   if (!a || !b) return false;
-  const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b, bytes = count * 8;
-  return pa < pb + bytes && pb < pa + bytes;
+  const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
+  return pa < pb + nb * 8 && pb < pa + na * 8;
+}
+
+// The top-level Rinv12 block that the factor skipped (complete_inv = 0, top node split at s1), rebuilt in Ri with the two products the
+// factor issues for it (cholinv_local.cu), with the same kernel, flags and shapes: T^T = R12^T Rinv11^T into W's lower-left block, then
+// Rinv12 = -(T^T)^T Rinv22.  RiT holds Rinv11^T on entry; on return its lower-left block holds Rinv12^T.  R is staged in and unpacked
+// into the factor's workspace "Rm".
+static capital_status_t rebuild_rinv12(capital_ctx* ctx, cudaStream_t st, int64_t L, int split, bool packed, const double* R_local,
+                                       size_t count, double* Ri, double* RiT, double* W, int64_t ld) {
+  const int64_t s1 = L >> split, s2 = L - s1;
+  const double* dR;
+  double* Rm;
+  CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Rm));
+  CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+  if (packed) CAP_TRY(unpack_upper(ctx, st, L, dR, Rm, ld));
+  else CAP_TRY(triu_copy(ctx, st, L, dR, L, Rm, ld, 0));
+  CAP_TRY(gemm_tn(ctx, st, s2, s1, s1, 1.0, Rm + s1 * ld, ld, RiT, ld, 0.0, W + s1, ld, CAPITAL_GEMM_B_LOWER));                     // T^T
+  CAP_TRY(gemm_tn(ctx, st, s1, s2, s2, -1.0, W + s1, ld, Ri + s1 * ld + s1, ld, 0.0, Ri + s1 * ld, ld, CAPITAL_GEMM_B_UPPER));  // Rinv12
+  return transpose_block(ctx, st, s1, s2, Ri + s1 * ld, ld, RiT + s1, ld, 1.0);
 }
 
 // A^-1 = Rinv Rinv^T from the factor's outputs: one DMMA product of Rinv^T (lower) with itself, upper tiles only, tile (i, j) running
@@ -721,8 +769,8 @@ capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n, const 
   const int64_t Lc = n > 0 ? ceil_div(n, std::max(ctx->grid.d, 1)) : 0;
   const size_t count = packed ? (size_t)Lc * (Lc + 1) / 2 : (size_t)Lc * Lc;
   if (!args || !Rinv_local || !Ainv_local || n <= 0 || args->split <= 0 || args->dir != 'U' ||
-      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED) || overlaps(Ainv_local, Rinv_local, count) ||
-      overlaps(Ainv_local, R_local, count)) {
+      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED) || overlaps(Ainv_local, count, Rinv_local, count) ||
+      overlaps(Ainv_local, count, R_local, count)) {
     ctx->set_error("cholinv::inverse: invalid arguments (Rinv and Ainv non-null, Ainv not overlapping R or Rinv, split > 0 and dir == 'U', "
                    "packed upper or rect)");
     return CAPITAL_ERR_INVALID;
@@ -748,18 +796,7 @@ capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n, const 
   if (packed) CAP_TRY(unpack_upper(ctx, st, L, dRi, Ri, ld));
   else CAP_TRY(triu_copy(ctx, st, L, dRi, L, Ri, ld, 0));
   CAP_TRY(transpose_block(ctx, st, L, L, Ri, ld, RiT, ld, 1.0));  // Rinv^T: lower, exact zeros above the diagonal
-  if (skipped) {
-    const int64_t s1 = L >> args->split, s2 = L - s1;
-    const double* dR;
-    double* Rm;
-    CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Rm));
-    CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
-    if (packed) CAP_TRY(unpack_upper(ctx, st, L, dR, Rm, ld));
-    else CAP_TRY(triu_copy(ctx, st, L, dR, L, Rm, ld, 0));
-    CAP_TRY(gemm_tn(ctx, st, s2, s1, s1, 1.0, Rm + s1 * ld, ld, RiT, ld, 0.0, W + s1, ld, CAPITAL_GEMM_B_LOWER));                     // T^T
-    CAP_TRY(gemm_tn(ctx, st, s1, s2, s2, -1.0, W + s1, ld, Ri + s1 * ld + s1, ld, 0.0, Ri + s1 * ld, ld, CAPITAL_GEMM_B_UPPER));  // Rinv12
-    CAP_TRY(transpose_block(ctx, st, s1, s2, Ri + s1 * ld, ld, RiT + s1, ld, 1.0));
-  }
+  if (skipped) CAP_TRY(rebuild_rinv12(ctx, st, L, (int)args->split, packed, R_local, count, Ri, RiT, W, ld));
   // upper tiles of (Rinv^T)^T Rinv^T; the lower-left T^T scratch in W is overwritten or never read
   CAP_TRY(gemm_tn(ctx, st, L, L, L, 1.0, RiT, ld, RiT, ld, 0.0, W, ld,
                   CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER));
@@ -768,6 +805,72 @@ capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n, const 
   else CAP_TRY(sym_merge(ctx, st, L, W, ld, W, ld, true, dOut, L, 0, 0, 1));  // the lower half is the upper one's mirror, bit for bit
   if (dOut != Ainv_local) {
     CAP_TRY(cap_stage_out_end(ctx, Ainv_local, count, dOut));
+    CAP_CUDA(cudaStreamSynchronize(st));
+  }
+  return CAPITAL_OK;
+}
+
+// A x = lambda B x with B = R^T R reduced to C y = lambda y, C = Rinv^T A Rinv (LAPACK dsygst, itype 1), in n^3 DMMA flops by LAPACK's
+// split A = U + U^T, U = triu(A) with its diagonal halved, C = M + M^T with M = Rinv^T U Rinv:
+//   V = U Rinv = (U^T)^T Rinv                 A_LOWER | B_UPPER | C_UPPER   n^3 / 3   (upper triangular: two upper factors)
+//   C_upper = Rinv^T V + V^T Rinv             A_UPPER | B_UPPER | C_UPPER   2 n^3 / 3, one launch with two operand classes
+// U^T is A's lower triangle with its diagonal halved (exact), so only that triangle of A is read.  A skipped top-level Rinv12 is rebuilt
+// first, as the inverse does.  The only buffers are the factor's four workspaces: Ri = Rinv, RiT = U^T (Rinv11^T for a rebuild first),
+// W = V (zeroed: the C_UPPER product leaves the strict lower part of its diagonal tiles unwritten, and the next product reads whole
+// diagonal tiles), Rm = C (R for a rebuild first).
+capital_status_t capital_cholinv_sygst_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                           const double* R_local, const double* Rinv_local, const double* A_local, double* C_local) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int64_t Lc = n > 0 ? ceil_div(n, std::max(ctx->grid.d, 1)) : 0;
+  const size_t count = packed ? (size_t)Lc * (Lc + 1) / 2 : (size_t)Lc * Lc, a_count = (size_t)Lc * Lc;
+  if (!args || !Rinv_local || !A_local || !C_local || n <= 0 || args->split <= 0 || args->dir != 'U' ||
+      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED) || overlaps(C_local, count, Rinv_local, count) ||
+      overlaps(C_local, count, R_local, count) || overlaps(C_local, count, A_local, a_count)) {
+    ctx->set_error("cholinv::sygst: invalid arguments (Rinv, A and C non-null, C not overlapping A, R or Rinv, split > 0 and dir == 'U', "
+                   "packed upper or rect)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  const capital_grid_t& g = ctx->grid;
+  if (g.size > 1) return dist_cholinv_sygst(ctx, n, args, structure, R_local, Rinv_local, A_local, C_local);
+  const int64_t L = n, ld = round_up(L, 16);
+  const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
+  const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::sygst: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  double *W, *Ri, *RiT, *Cm, *dOut;
+  CAP_TRY(ctx->workspace("W", (size_t)ld * L * 8, (void**)&W));
+  CAP_TRY(ctx->workspace("Ri", (size_t)ld * L * 8, (void**)&Ri));
+  CAP_TRY(ctx->workspace("RiT", (size_t)ld * L * 8, (void**)&RiT));
+  const double* dRi;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, count, "Rinv_out", &dRi));
+  if (packed) CAP_TRY(unpack_upper(ctx, st, L, dRi, Ri, ld));
+  else CAP_TRY(triu_copy(ctx, st, L, dRi, L, Ri, ld, 0));
+  if (skipped) {
+    const int64_t s1 = L >> args->split;
+    CAP_TRY(transpose_block(ctx, st, s1, s1, Ri, ld, RiT, ld, 1.0));  // Rinv11^T, the rebuild's only use of RiT's upper-left block
+    CAP_TRY(rebuild_rinv12(ctx, st, L, (int)args->split, packed, R_local, count, Ri, RiT, W, ld));
+  }
+  CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Cm));
+  const double* dA;
+  CAP_TRY(cap_stage_in(ctx, A_local, a_count, "A_in", &dA));
+  CAP_TRY(tril_half_copy(ctx, st, L, dA, L, RiT, ld, 0, 0, 1));  // U^T
+  CAP_CUDA(cudaMemsetAsync(W, 0, (size_t)ld * L * 8, st));
+  CAP_TRY(gemm_tn(ctx, st, L, L, L, 1.0, RiT, ld, Ri, ld, 0.0, W, ld, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));
+  GemmOperands ops;
+  ops.ncls = 2; ops.lda = ops.ldb = ld;
+  ops.A[0] = Ri; ops.B[0] = W;  // Rinv^T V
+  ops.A[1] = W; ops.B[1] = Ri;  // V^T Rinv
+  CAP_TRY(gemm_tn_x(ctx, st, L, L, L, 1.0, ops, 0.0, Cm, ld, CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER, 0, nullptr));
+  CAP_TRY(cap_stage_out_begin(ctx, C_local, count, "R_out", &dOut));
+  if (packed) CAP_TRY(pack_upper(ctx, st, L, Cm, ld, dOut, 0));
+  else CAP_TRY(sym_merge(ctx, st, L, Cm, ld, Cm, ld, true, dOut, L, 0, 0, 1));  // the lower half is the upper one's mirror, bit for bit
+  if (dOut != C_local) {
+    CAP_TRY(cap_stage_out_end(ctx, C_local, count, dOut));
     CAP_CUDA(cudaStreamSynchronize(st));
   }
   return CAPITAL_OK;

@@ -172,6 +172,10 @@ capital_status_t triu_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const d
 // global (y + d r, x + d c)), below it the mirror S, read transposed (s_trans: S(c, r), on one GPU S = U) or as it is
 capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* U, int64_t ldu, const double* S, int64_t lds,
                            bool s_trans, double* out, int64_t ldo, int x, int y, int d);
+// n x n local block of U^T, U = triu(A) with its diagonal halved (sygst's A = U + U^T): the global lower triangle of the symmetric A
+// (local (r, c) is global (y + d r, x + d c)) with its diagonal times 1/2, zeros above it.  The global upper triangle is never read.
+capital_status_t tril_half_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst, int64_t ldd,
+                                int x, int y, int d);
 capital_status_t gen_symmetric(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,
                                int64_t n_global, int x, int y, int d, int diag_dom);
 capital_status_t gen_random(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,

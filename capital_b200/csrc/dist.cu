@@ -1213,9 +1213,11 @@ capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, 
 // rows = y), and sum the partials over all ranks with peer_allreduce_sum, which adds them in rank order -- X is bit-identical
 // everywhere.  The c layers split each window's columns into shares of equal triangle area, so every factor element enters the sum
 // exactly once.
+// A half alone (mode SOLVE_RINVT / SOLVE_RINV: capital_cholinv_apply_rinv_f64) runs that half's steps, with the same shares and the
+// same all-reduce slot set (signature cholsolve:n), so switching between solve and apply costs no arena clear.
 capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                     const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
-                                    double* X, int64_t ldx) {
+                                    double* X, int64_t ldx, int mode) {
   CAP_TRY(need_comm(ctx));
   Dist D;
   CAP_TRY(dist_setup(D, ctx, false));
@@ -1275,21 +1277,31 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
     const int64_t o0 = d * (trans ? c0 : r0), o1 = d * (trans ? c1 : r1);
     return panel_add(ctx, st, o1 - o0, w, S + o0, n, Cin ? Cin + o0 : nullptr, ldcin, Out + o0, ldo);
   };
+  // first half: T = R^-T Bp
+  auto half_t = [&](const double* Bp, int64_t w) -> capital_status_t {
+    if (!skipped) return step(dRi, true, 0, L, 0, L, w, 1.0, Bp, ldb, nullptr, 0, T, n);  // Y = Rinv^T B
+    CAP_TRY(step(dRi, true, 0, s1, 0, s1, w, 1.0, Bp, ldb, nullptr, 0, T, n));  // Y1
+    CAP_TRY(step(dR, true, 0, s1, s1, L, w, -1.0, T, n, Bp, ldb, T2, n));       // B2 - R12^T Y1
+    return step(dRi, true, s1, L, s1, L, w, 1.0, T2, n, nullptr, 0, T, n);      // Y2
+  };
+  // second half: Xp = R^-1 Yp.  Every step writes its output only after the all-reduce of its input, so Xp may alias Yp
+  auto half_n = [&](const double* Yp, int64_t ldy, double* Xp, int64_t w) -> capital_status_t {
+    if (!skipped) return step(dRi, false, 0, L, 0, L, w, 1.0, Yp, ldy, nullptr, 0, Xp, ldx);  // X = Rinv Y
+    CAP_TRY(step(dRi, false, s1, L, s1, L, w, 1.0, Yp, ldy, nullptr, 0, Xp, ldx)); // X2
+    CAP_TRY(step(dR, false, 0, s1, s1, L, w, -1.0, Xp, ldx, Yp, ldy, T2, n));      // Y1 - R12 X2
+    return step(dRi, false, 0, s1, 0, s1, w, 1.0, T2, n, nullptr, 0, Xp, ldx);     // X1
+  };
   for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
     const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
     const double* Bp = dB + p0 * ldb;
     double* Xp = dX + p0 * ldx;
-    if (!skipped) {
-      CAP_TRY(step(dRi, true, 0, L, 0, L, w, 1.0, Bp, ldb, nullptr, 0, T, n));    // Y = Rinv^T B
-      CAP_TRY(step(dRi, false, 0, L, 0, L, w, 1.0, T, n, nullptr, 0, Xp, ldx));   // X = Rinv Y
-    } else {
-      CAP_TRY(step(dRi, true, 0, s1, 0, s1, w, 1.0, Bp, ldb, nullptr, 0, T, n));  // Y1
-      CAP_TRY(step(dR, true, 0, s1, s1, L, w, -1.0, T, n, Bp, ldb, T2, n));       // B2 - R12^T Y1
-      CAP_TRY(step(dRi, true, s1, L, s1, L, w, 1.0, T2, n, nullptr, 0, T, n));    // Y2
-      CAP_TRY(step(dRi, false, s1, L, s1, L, w, 1.0, T, n, nullptr, 0, Xp, ldx)); // X2
-      CAP_TRY(step(dR, false, 0, s1, s1, L, w, -1.0, Xp, ldx, T, n, T2, n));      // Y1 - R12 X2
-      CAP_TRY(step(dRi, false, 0, s1, 0, s1, w, 1.0, T2, n, nullptr, 0, Xp, ldx)); // X1
+    if (mode == SOLVE_RINV) {
+      CAP_TRY(half_n(Bp, ldb, Xp, w));
+      continue;
     }
+    CAP_TRY(half_t(Bp, w));
+    if (mode == SOLVE_FULL) CAP_TRY(half_n(T, n, Xp, w));
+    else CAP_TRY(panel_add(ctx, st, n, w, T, n, nullptr, 0, Xp, ldx));
   }
   if (x_host) {
     CAP_CUDA(cudaMemcpy2DAsync(X, (size_t)ldx * 8, dX, (size_t)ldx * 8, (size_t)n * 8, (size_t)nrhs, cudaMemcpyDeviceToHost, st));
@@ -1321,6 +1333,44 @@ size_t inverse_layout(Dist& D, Inv& v, char* base) {
   return lay.off;
 }
 
+// The top-level Rinv12 block that the factor skipped, rebuilt in Ri (which holds the factor's Rinv, Rinv12 zero) with the two products
+// of invoke for that block, with its shapes, flags and chunking:
+//   T^T = R12^T Rinv11^T (B = RiT11, lower triangular), then Rinv12 = -(T^T)^T Rinv22 (B = Ri22, upper triangular).
+// dR: the factor's R on the device, unpacked into R first.  Every block of Ri travels once: in the roles the rebuild needs, plus
+// `ri_roles`.  whole_rit: RiT = Rinv^T entirely afterwards, every block pushed to its X and Y consumers (the inverse's operand);
+// otherwise only RiT11, the rebuild's own operand, is built and pushed.
+capital_status_t rebuild_rinv12(Dist& D, DMat& Ri, DMat& RiT, DMat& R, DMat& W, const double* dR, bool packed, int zdiag, int ri_roles,
+                                bool whole_rit) {
+  capital_ctx* ctx = D.ctx;
+  const capital_grid_t& g = D.g;
+  const int64_t L = D.L, ld = D.ld;
+  const int cs = S_CHAIN;
+  const int64_t s1 = L >> D.split, s2 = L - s1;
+  const int rit_roles = whole_rit ? ROLE_X | ROLE_Y : ROLE_Y;
+  D.wr(cs, D.me, R.own, ld, L, L);
+  if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dR, R.own, ld));
+  else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dR, L, R.own, ld, zdiag));
+  // the diagonal blocks of Rinv are final: their transposes travel first (RiT12 stays zero: it is never written, nor pushed)
+  CAP_TRY(push(D, Q_CHAIN, cs, Ri, 0, 0, s1, s1, ROLE_T | ri_roles, nullptr));
+  CAP_TRY(push(D, Q_CHAIN, cs, Ri, s1, s1, s2, s2, ROLE_Y | (whole_rit ? ROLE_T : 0) | ri_roles, nullptr));
+  CAP_TRY(push(D, Q_CHAIN, cs, R, 0, s1, s1, s2, ROLE_X, nullptr));
+  CAP_TRY(transpose_dist(D, Q_CHAIN, Ri, 0, 0, s1, s1, nullptr, RiT.own, ld));
+  if (whole_rit) CAP_TRY(transpose_dist(D, Q_CHAIN, Ri, s1, s1, s2, s2, nullptr, RiT.own + s1 * ld + s1, ld));
+  CAP_TRY(push(D, Q_CHAIN, cs, RiT, 0, 0, s1, s1, rit_roles, nullptr));
+  if (whole_rit) CAP_TRY(push(D, Q_CHAIN, cs, RiT, s1, s1, s2, s2, rit_roles, nullptr));
+  CAP_TRY(product(D, Q_CHAIN, s2, s1, s1, 1.0, Win{&R, 0, s1}, Win{&RiT, 0, 0}, 0.0, Win{&W, s1, 0}, CAPITAL_GEMM_B_LOWER));
+  CAP_TRY(push(D, Q_CHAIN, cs, W, s1, 0, s2, s1, ROLE_X, nullptr));
+  const int nch = (g.size > 1 && D.d > 1 && s2 >= D.chunk_min) ? D.chunks : 1;
+  Token tRi12;
+  CAP_TRY(product_pushed(D, Q_CHAIN, s1, s2, s2, -1.0, Win{&W, s1, 0}, Win{&Ri, s1, s1}, 0.0, Win{&Ri, 0, s1}, CAPITAL_GEMM_B_UPPER,
+                         nullptr, nullptr, (whole_rit ? ROLE_T : 0) | ri_roles, &tRi12, nch));
+  if (whole_rit) {
+    CAP_TRY(transpose_dist(D, Q_CHAIN, Ri, 0, s1, s1, s2, &tRi12, RiT.own + s1, ld));
+    CAP_TRY(push(D, Q_CHAIN, cs, RiT, s1, 0, s2, s1, rit_roles, nullptr));
+  }
+  return CAPITAL_OK;
+}
+
 // dRi (and dR when `skipped`): the factor's outputs on the device; dOut: the local output block.  None is touched in a dry run.
 capital_status_t inverse_run(Dist& D, Inv& v, bool skipped, capital_structure_t structure, const double* dRi, const double* dR,
                              double* dOut) {
@@ -1342,28 +1392,7 @@ capital_status_t inverse_run(Dist& D, Inv& v, bool skipped, capital_structure_t 
     CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, 0, L, L, nullptr, v.RiT.own, ld));
     CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
   } else {
-    const int64_t s1 = L >> D.split, s2 = L - s1;
-    D.wr(cs, D.me, v.R.own, ld, L, L);
-    if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dR, v.R.own, ld));
-    else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dR, L, v.R.own, ld, zdiag));
-    // the diagonal blocks of Rinv are final: their transposes travel first (RiT12 stays zero: it is never written, nor pushed)
-    CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, 0, 0, s1, s1, ROLE_T, nullptr));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, s1, s1, s2, s2, ROLE_Y | ROLE_T, nullptr));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.R, 0, s1, s1, s2, ROLE_X, nullptr));
-    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, 0, s1, s1, nullptr, v.RiT.own, ld));
-    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, s1, s1, s2, s2, nullptr, v.RiT.own + s1 * ld + s1, ld));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, 0, 0, s1, s1, ROLE_X | ROLE_Y, nullptr));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, s1, s1, s2, s2, ROLE_X | ROLE_Y, nullptr));
-    // the two products of invoke for the top-level block, with its shapes, flags and chunking:
-    //   T^T = R12^T Rinv11^T (B = RiT11, lower triangular), then Rinv12 = -(T^T)^T Rinv22 (B = Ri22, upper triangular)
-    CAP_TRY(product(D, Q_CHAIN, s2, s1, s1, 1.0, Win{&v.R, 0, s1}, RiT0, 0.0, Win{&v.W, s1, 0}, CAPITAL_GEMM_B_LOWER));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.W, s1, 0, s2, s1, ROLE_X, nullptr));
-    const int nch = (g.size > 1 && D.d > 1 && s2 >= D.chunk_min) ? D.chunks : 1;
-    Token tRi12;
-    CAP_TRY(product_pushed(D, Q_CHAIN, s1, s2, s2, -1.0, Win{&v.W, s1, 0}, Win{&v.Ri, s1, s1}, 0.0, Win{&v.Ri, 0, s1}, CAPITAL_GEMM_B_UPPER,
-                           nullptr, nullptr, ROLE_T, &tRi12, nch));
-    CAP_TRY(transpose_dist(D, Q_CHAIN, v.Ri, 0, s1, s1, s2, &tRi12, v.RiT.own + s1, ld));
-    CAP_TRY(push(D, Q_CHAIN, cs, v.RiT, s1, 0, s2, s1, ROLE_X | ROLE_Y, nullptr));
+    CAP_TRY(rebuild_rinv12(D, v.Ri, v.RiT, v.R, v.W, dR, packed, zdiag, 0, true));
   }
   // the upper half of A^-1 = (Rinv^T)^T Rinv^T: tile (i, j) runs k from max(i, j)
   CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, RiT0, RiT0, 0.0, Win{&v.C, 0, 0},
@@ -1416,6 +1445,113 @@ extern "C" capital_status_t capital_dist_trace_cholinv_inverse(const capital_gri
     const bool skipped = args->complete_inv == 0 && node_splits(D, D.L);
     capital_status_t st = CAPITAL_OK;
     for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = inverse_run(D, v, skipped, CAPITAL_RECT, nullptr, nullptr, nullptr);
+    return st;
+  });
+}
+
+// cholinv::sygst on the grid: C = Rinv^T A Rinv by LAPACK's split A = U + U^T (api.cu, capital_cholinv_sygst_f64), as three distributed
+// products with the depth reduction in the epilogue: V = (U^T)^T Rinv, then C_upper = Rinv^T V, then C_upper += V^T Rinv (beta = 1: the
+// sum order is fixed).  U^T's local block is the rank's block of A masked to the global lower triangle, diagonal halved (tril_half_copy);
+// it is lower triangular on ranks with x <= y and strictly lower on the others, so A_LOWER holds locally as it does for R and Rinv.
+// Where the factor skipped the top-level Rinv12, it is rebuilt first (rebuild_rinv12).  The rect output's lower half is the transpose
+// partner's upper half, merged in (sym_merge).  Every window of a mirror slot is pushed at most once per call.
+namespace {
+struct Gst {
+  DMat Ri, RiT, R, W, Au, V, C, Ct;
+};
+// one layout for complete and skipped Rinv12 (signature cholinv_gst:L).  V's strict lower part is never written (C_UPPER products), so it
+// keeps the zeros of the arena's clear, which the next product's whole diagonal tiles read.
+size_t sygst_layout(Dist& D, Gst& v, char* base) {
+  Layout lay(base);
+  const int64_t L = D.L, ld = D.ld;
+  layout_mat(lay, D, v.Ri, ld, L, ROLE_X | ROLE_Y | ROLE_T, true);  // X, Y: the products' Rinv; T: Rinv11 for a rebuild's RiT11
+  layout_mat(lay, D, v.RiT, ld, L, ROLE_Y, false);  // Rinv11^T of a rebuilt Rinv12
+  layout_mat(lay, D, v.R, ld, L, ROLE_X, false);    // R12 of a rebuilt Rinv12
+  layout_mat(lay, D, v.W, ld, L, ROLE_X, false);    // T^T of a rebuilt Rinv12 (lower-left block)
+  layout_mat(lay, D, v.Au, ld, L, ROLE_X, false);   // U^T
+  layout_mat(lay, D, v.V, ld, L, ROLE_X | ROLE_Y, true);
+  layout_mat(lay, D, v.C, ld, L, ROLE_T, false);    // upper half of C; T: the partner's lower half of a rect output
+  layout_mat(lay, D, v.Ct, ld, L, 0, false);
+  layout_exchange(lay, D, Q_CHAIN, L, L);
+  return lay.off;
+}
+
+// dRi, dA (and dR when `skipped`): the factors and A on the device; dOut: the local output block.  None is touched in a dry run.
+capital_status_t sygst_run(Dist& D, Gst& v, bool skipped, capital_structure_t structure, const double* dRi, const double* dR,
+                           const double* dA, double* dOut) {
+  capital_ctx* ctx = D.ctx;
+  const capital_grid_t& g = D.g;
+  const int64_t L = D.L, ld = D.ld;
+  const int cs = S_CHAIN;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int zdiag = g.y > g.x ? 1 : 0;  // there the local diagonal lies below the global one
+  ctx->comm_used = 0;
+  CAP_TRY(fork_streams(D));
+  if (!D.dry) CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), D.strm(cs)));
+  D.wr(cs, D.me, v.Ri.own, ld, L, L);
+  if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dRi, v.Ri.own, ld));
+  else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dRi, L, v.Ri.own, ld, zdiag));
+  if (!skipped) CAP_TRY(push(D, Q_CHAIN, cs, v.Ri, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
+  else CAP_TRY(rebuild_rinv12(D, v.Ri, v.RiT, v.R, v.W, dR, packed, zdiag, ROLE_X | ROLE_Y, false));
+  D.wr(cs, D.me, v.Au.own, ld, L, L);
+  DO(D, cs, tril_half_copy(ctx, D.strm(cs), L, dA, L, v.Au.own, ld, g.x, g.y, g.d));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.Au, 0, 0, L, L, ROLE_X, nullptr));
+  const Win Ri0{&v.Ri, 0, 0}, V0{&v.V, 0, 0}, C0{&v.C, 0, 0};
+  const int tri = CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER;
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, Win{&v.Au, 0, 0}, Ri0, 0.0, V0,
+                  CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));  // V = U Rinv
+  CAP_TRY(push(D, Q_CHAIN, cs, v.V, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, Ri0, V0, 0.0, C0, tri));  // Rinv^T V
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, V0, Ri0, 1.0, C0, tri));  // + V^T Rinv
+  if (packed) {
+    D.rd(cs, v.C.own, ld, L, L);
+    DO(D, cs, pack_upper(ctx, D.strm(cs), L, v.C.own, ld, dOut, zdiag));
+  } else {
+    CAP_TRY(push(D, Q_CHAIN, cs, v.C, 0, 0, L, L, ROLE_T, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.C, 0, 0, L, L, nullptr, v.Ct.own, ld));
+    D.rd(cs, v.C.own, ld, L, L);
+    D.rd(cs, v.Ct.own, ld, L, L);
+    DO(D, cs, sym_merge(ctx, D.strm(cs), L, v.C.own, ld, v.Ct.own, ld, false, dOut, L, g.x, g.y, g.d));
+  }
+  return join_streams(D);
+}
+}  // namespace
+
+capital_status_t dist_cholinv_sygst(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                    const double* R_local, const double* Rinv_local, const double* A_local, double* C_local) {
+  CAP_TRY(need_comm(ctx));
+  Dist D;
+  CAP_TRY(dist_setup(D, ctx, false));
+  CAP_TRY(cholinv_shape(D, n, args));
+  const int64_t L = D.L;
+  const bool skipped = args->complete_inv == 0 && node_splits(D, L);  // the factor's predicate (cholinv_run)
+  if (skipped && !R_local) {
+    ctx->set_error("cholinv::sygst: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
+    return CAPITAL_ERR_INVALID;
+  }
+  const size_t count = structure == CAPITAL_UPPERTRI_PACKED ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
+  const double *dRi, *dR = nullptr, *dA;
+  double* dOut;
+  CAP_TRY(cap_stage_in(ctx, Rinv_local, count, "Rinv_out", &dRi));
+  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+  CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
+  CAP_TRY(cap_stage_out_begin(ctx, C_local, count, "gst_out", &dOut));
+  Gst v;
+  CAP_TRY(arena_layout(ctx, "cholinv_gst:" + std::to_string(L), [&](char* base) { return sygst_layout(D, v, base); }));
+  CAP_TRY(sygst_run(D, v, skipped, structure, dRi, dR, dA, dOut));
+  CAP_TRY(cap_stage_out_end(ctx, C_local, count, dOut));
+  return cap_check_info(ctx);
+}
+
+// Dry run of two consecutive cholinv::sygst calls (rect output) on one rank of a grid.
+extern "C" capital_status_t capital_dist_trace_cholinv_sygst(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args,
+                                                              int64_t* out, int64_t cap_records, int64_t* n_records) {
+  return dry_trace(grid, n, args, out, cap_records, n_records, [&](Dist& D, char* arena) {
+    Gst v;
+    sygst_layout(D, v, arena);
+    const bool skipped = args->complete_inv == 0 && node_splits(D, D.L);
+    capital_status_t st = CAPITAL_OK;
+    for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = sygst_run(D, v, skipped, CAPITAL_RECT, nullptr, nullptr, nullptr, nullptr);
     return st;
   });
 }

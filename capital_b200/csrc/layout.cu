@@ -92,6 +92,21 @@ __global__ void sym_merge_kernel(int n, const double* U, long long ldu, const do
   }
 }
 
+// The operand U^T of sygst's split A = U + U^T (U = triu(A) with its diagonal halved): dst(r, c) = A(r, c) where the GLOBAL position
+// (y + d r, x + d c) lies strictly below the diagonal, A(r, c) / 2 on it, 0 above it.  Entries above the global diagonal are never
+// read, so whatever they hold (NaN included) cannot reach the result.
+__global__ void tril_half_copy_kernel(long long n, const double* src, long long lds, double* dst, long long ldd, int x, int y, int d) {
+  for (long long c = blockIdx.x; c < n; c += gridDim.x) {
+    const double* s = src + c * lds;
+    double* o = dst + c * ldd;
+    const long long gc = x + (long long)d * c;
+    for (long long r = threadIdx.x; r < n; r += blockDim.x) {
+      const long long gr = y + (long long)d * r;
+      o[r] = gr > gc ? s[r] : (gr == gc ? 0.5 * s[r] : 0.0);
+    }
+  }
+}
+
 // drand48: X0 = seed<<16 | 0x330E ; X1 = (a X0 + c) mod 2^48 ; value = X1 / 2^48  (structure.hpp:80-85 re-seeds per element)
 __device__ __forceinline__ double drand48_first(unsigned long long seed) {
   const unsigned long long a = 0x5DEECE66DULL, c = 0xBULL, m48 = (1ULL << 48) - 1;
@@ -296,6 +311,13 @@ capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const d
   if (n <= 0) return CAPITAL_OK;
   dim3 grid((unsigned)ceil_div(n, TP), (unsigned)ceil_div(n, TP)), block(TP, 8);
   sym_merge_kernel<<<grid, block, 0, st>>>((int)n, U, ldu, S, lds, s_trans ? 1 : 0, out, ldo, x, y, d);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t tril_half_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst, int64_t ldd,
+                                int x, int y, int d) {
+  if (n <= 0) return CAPITAL_OK;
+  tril_half_copy_kernel<<<(int)(n < ctx->num_sms * 8 ? n : ctx->num_sms * 8), 256, 0, st>>>(n, src, lds, dst, ldd, x, y, d);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

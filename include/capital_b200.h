@@ -138,6 +138,9 @@ capital_status_t capital_dist_trace_cacqr(const capital_grid_t* grid, int64_t m_
 /* The same for two consecutive capital_cholinv_inverse_f64 calls (rect output) on a square grid. */
 capital_status_t capital_dist_trace_cholinv_inverse(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
                                                     int64_t* out, int64_t cap_records, int64_t* n_records);
+/* The same for two consecutive capital_cholinv_sygst_f64 calls (rect output) on a square grid. */
+capital_status_t capital_dist_trace_cholinv_sygst(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
+                                                  int64_t* out, int64_t cap_records, int64_t* n_records);
 
 /* ---- generators (device kernels; bit-exact with the reference's drand48-based ones) ---------- */
 /* matrix::distribute_symmetric(x, y, d, d, key, diagonallyDominant) -- structure.hpp:69-103. */
@@ -173,6 +176,14 @@ capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_
 capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
                                            capital_structure_t structure, const double* R_local, const double* Rinv_local,
                                            int64_t nrhs, const double* B, int64_t ldb, double* X, int64_t ldx);
+/* One half of the solve alone: trans = 0: X = R^-1 B (the back-transform x = R^-1 y of capital_cholinv_sygst_f64); trans = 1:
+ * X = R^-T B (whitening).  Arguments, conventions and guarantees as capital_cholinv_solve_f64 (X may alias B).  Rinv complete: one pass
+ * over the triangle per panel.  Rinv12 skipped: trans = 1 runs the solve's first three steps (Y1, B2 - R12^T Y1, Y2), trans = 0 its
+ * last three (X2, Y1 - R12 X2, X1).  Each step is the solve's own, so apply_rinv(0) after apply_rinv(1) gives the solve's bits.  On a
+ * grid it uses the solve's all-reduce slots: switching between solve and apply costs no arena clear. */
+capital_status_t capital_cholinv_apply_rinv_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                                capital_structure_t structure, const double* R_local, const double* Rinv_local,
+                                                int trans, int64_t nrhs, const double* B, int64_t ldb, double* X, int64_t ldx);
 
 /* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
  * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
@@ -187,6 +198,20 @@ capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n_global, c
 capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
                                              capital_structure_t structure, const double* R_local, const double* Rinv_local,
                                              double* Ainv_local);
+/* Generalized symmetric-definite eigenproblem A x = lambda B x, reduced to standard form with the outputs of
+ * capital_cholinv_factor_f64 for B = R^T R (LAPACK dsygst, itype 1, upper): C = R^-T A R^-1, so that C y = lambda y and x = R^-1 y
+ * (capital_cholinv_apply_rinv_f64 with trans = 0).  Collective on a grid, with the arguments of the factor of B.  A_local: the rank's
+ * L x L rect block of the symmetric A (as the generator writes it); only its GLOBAL lower triangle, the diagonal included, is read.
+ * R_local / Rinv_local as for capital_cholinv_inverse_f64 (R only for a skipped top-level Rinv12, rebuilt first; NULL otherwise).
+ * C_local: the rank's L x L block in `structure`, written exactly as the inverse writes A^-1: packed upper (zeros on the
+ * local-diagonal slots of ranks with y > x) or the full rect block, exactly symmetric.  Identical on the c layers; deterministic.
+ * n^3 DMMA flops (LAPACK's split A = U + U^T): V = U R^-1, then C = R^-T V + V^T R^-1, upper tiles only.  C must not overlap A, R
+ * or Rinv.  Host or device pointers.  One GPU: enqueued on the context stream, synchronous only when C is a host pointer; with device
+ * pointers the only device memory is the factor's own four L x L workspaces.  Grid: synchronous; the products use the peer arena, so
+ * the next factor call re-clears it.  CAPITAL_ERR_UNSUPPORTED when d does not divide n on a grid. */
+capital_status_t capital_cholinv_sygst_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                           capital_structure_t structure, const double* R_local, const double* Rinv_local,
+                                           const double* A_local, double* C_local);
 /* inverse::validate -- test/inverse/validate.hpp:7-34: ||A Ainv - I||_F / ||I||_F over the whole matrix, computed on the device(s),
  * the diagonal taken by GLOBAL index.  A_local: the full symmetric rect local block (as the generator writes it); Ainv_local: as
  * capital_cholinv_inverse_f64 wrote it in `structure`. */
