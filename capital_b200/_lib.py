@@ -13,10 +13,11 @@ GEMM_A_UPPER, GEMM_A_LOWER, GEMM_B_UPPER, GEMM_B_LOWER, GEMM_C_UPPER = 1, 2, 4, 
 
 EXPORTS = [  # every symbol include/capital_b200.h declares
     "capital_grid_square", "capital_grid_rect", "capital_cholinv_bc_dimension", "capital_create",
-    "capital_comm_unique_id", "capital_comm_init", "capital_comm_init_host", "capital_peer_wait_mode", "capital_set_peer_wait_mode", "capital_dist_trace_cholinv", "capital_dist_trace_cacqr", "capital_dist_trace_cholinv_inverse", "capital_dist_trace_cholinv_sygst", "capital_destroy", "capital_last_error", "capital_get_counters",
+    "capital_comm_unique_id", "capital_comm_init", "capital_comm_init_host", "capital_peer_wait_mode", "capital_set_peer_wait_mode", "capital_dist_trace_cholinv", "capital_dist_trace_cacqr", "capital_dist_trace_cholinv_inverse", "capital_dist_trace_cholinv_sygst", "capital_dist_trace_cholinv_sygst_ab", "capital_destroy", "capital_last_error", "capital_get_counters",
     "capital_reset_counters", "capital_synchronize", "capital_set_stream", "capital_release_workspace", "capital_last_factor_ms", "capital_profile_begin", "capital_profile_end", "capital_probe_dmma_f64", "capital_blas_gemm_tn_tf32", "capital_set_trailing_precision", "capital_tf32_stats", "capital_timeline_begin", "capital_timeline_end", "capital_set_overlap", "capital_distribute_symmetric_f64",
     "capital_distribute_random_f64", "capital_cholinv_factor_f64", "capital_cholinv_residual_f64", "capital_cholinv_solve_f64",
     "capital_cholinv_inverse_f64", "capital_cholinv_inverse_residual_f64", "capital_cholinv_sygst_f64", "capital_cholinv_apply_rinv_f64",
+    "capital_cholinv_sygst_ab_f64", "capital_cholinv_apply_r_f64",
     "capital_cacqr_factor_f64", "capital_cacqr_residual_f64", "capital_cacqr_apply_qt_f64", "capital_cacqr_apply_q_f64",
     "capital_cacqr_lstsq_f64", "capital_summa_gemm_tn_f64", "capital_blas_gemm_tn_f64",
     "capital_lapack_potrf_trtri_f64",
@@ -99,6 +100,9 @@ def lib() -> C.CDLL:
     L.capital_cholinv_sygst_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, vp, vp, vp]
     L.capital_cholinv_apply_rinv_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, vp, ci, i64, vp, i64, vp, i64]
     L.capital_dist_trace_cholinv_sygst.argtypes = [C.POINTER(Grid), i64, C.POINTER(CholinvArgs), C.POINTER(i64), i64, C.POINTER(i64)]
+    L.capital_cholinv_sygst_ab_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, vp, vp]
+    L.capital_cholinv_apply_r_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, ci, i64, vp, i64, vp, i64]
+    L.capital_dist_trace_cholinv_sygst_ab.argtypes = [C.POINTER(Grid), i64, C.POINTER(CholinvArgs), C.POINTER(i64), i64, C.POINTER(i64)]
     L.capital_cacqr_factor_f64.argtypes = [vp, vp, i64, i64, ci, C.POINTER(CholinvArgs), ci, vp, vp]
     L.capital_cacqr_residual_f64.argtypes = [vp, vp, i64, i64, vp, ci, vp, C.POINTER(dbl), C.POINTER(dbl)]
     L.capital_cacqr_apply_qt_f64.argtypes = [vp, i64, i64, vp, i64, vp, i64, vp, i64]

@@ -9,6 +9,9 @@
     C = cholinv.sygst(A2, args, topo)                                # C = R^-T A2 R^-1 for A2 x = l A x (capital_cholinv_sygst_f64)
     X = cholinv.apply_Rinv(args, Y, topo)                            # R^-1 Y, the back-transform (capital_cholinv_apply_rinv_f64)
     W = cholinv.apply_RinvT(args, B, topo)                           # R^-T B, whitening
+    C = cholinv.sygst(A2, args, topo, itype=2)                       # C = R A2 R^T for A2 A x = l x or A A2 x = l x (itype 3)
+    X = cholinv.apply_R(args, Z, topo)                               # R Z (capital_cholinv_apply_r_f64)
+    X = cholinv.apply_RT(args, Y, topo)                              # R^T Y, the itype 3 back-transform
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -136,12 +139,17 @@ def inverse(args: info, topo) -> torch.Tensor:
     return out
 
 
-def sygst(A: matrix, args: info, topo) -> torch.Tensor:
-    """A x = lambda B x reduced to C y = lambda y with the factors of a previous `factor(B, args, topo)` (capital_cholinv_sygst_f64,
-    LAPACK dsygst itype 1): C = R^-T A R^-1, and x = apply_Rinv(args, y, topo).  A: the symmetric matrix, a `matrix` shaped like the
-    factored B; only its global lower triangle (diagonal included) is read.  Returns the local block of C like `inverse` does: a flat
-    float64 tensor with args.Rinv's length and device (pinned on the host), packed upper when args.serialize, else the full, exactly
-    symmetric rect block.  The same bits on every layer of a grid."""
+def sygst(A: matrix, args: info, topo, itype: int = 1) -> torch.Tensor:
+    """A generalized symmetric-definite eigenproblem reduced to C y = lambda y with the factors of a previous `factor(B, args, topo)`,
+    B = R^T R (LAPACK dsygst, upper), with the same eigenvalues:
+      itype 1: A x = lambda B x,  C = R^-T A R^-1 (capital_cholinv_sygst_f64),    back-transform x = apply_Rinv(args, y, topo);
+      itype 2: A B x = lambda x,  C = R A R^T     (capital_cholinv_sygst_ab_f64), back-transform x = apply_Rinv(args, y, topo);
+      itype 3: B A x = lambda x,  C = R A R^T     (capital_cholinv_sygst_ab_f64), back-transform x = apply_RT(args, y, topo).
+    A: the symmetric matrix, a `matrix` shaped like the factored B; only its global lower triangle (diagonal included) is read.  Returns
+    the local block of C like `inverse` does: a flat float64 tensor with args.Rinv's length and device (pinned on the host), packed upper
+    when args.serialize, else the full, exactly symmetric rect block.  The same bits on every layer of a grid."""
+    if isinstance(itype, bool) or itype not in (1, 2, 3):
+        raise ValueError(f"cholinv.sygst: itype must be 1, 2 or 3, got {itype!r}")
     count = _check_factors(args, "sygst")
     if not isinstance(A, matrix) or A.num_rows_global != args.global_dim or A.num_columns_global != args.global_dim \
             or A.num_rows_local != args.local_dim or A.num_columns_local != args.local_dim:
@@ -152,13 +160,18 @@ def sygst(A: matrix, args: info, topo) -> torch.Tensor:
     out = torch.empty(count, dtype=torch.float64, device=dev, pin_memory=dev.type == "cpu")
     ctx = topo.context()
     cargs = args._c()
-    ctx.check(_lib.lib().capital_cholinv_sygst_f64(ctx.handle, args.global_dim, C.byref(cargs),
-                                                   _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
-                                                   args.R.data_ptr(), args.Rinv.data_ptr(), A.data.data_ptr(), out.data_ptr()))
+    structure = _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT
+    if itype == 1:
+        ctx.check(_lib.lib().capital_cholinv_sygst_f64(ctx.handle, args.global_dim, C.byref(cargs), structure,
+                                                       args.R.data_ptr(), args.Rinv.data_ptr(), A.data.data_ptr(), out.data_ptr()))
+    else:
+        ctx.check(_lib.lib().capital_cholinv_sygst_ab_f64(ctx.handle, args.global_dim, C.byref(cargs), structure,
+                                                          args.R.data_ptr(), A.data.data_ptr(), out.data_ptr()))
     return out
 
 
-def _apply_rinv(args: info, B: torch.Tensor, topo, trans: int, what: str) -> torch.Tensor:
+def _apply(args: info, B: torch.Tensor, topo, trans: int, what: str, factor_r: bool) -> torch.Tensor:
+    """X = op(F) B with F = R (factor_r) or Rinv: the right-hand-side checks and layout shared by the apply_* entry points"""
     _check_factors(args, what)
     if not isinstance(B, torch.Tensor) or B.dtype != torch.float64:
         raise ValueError(f"cholinv.{what}: B must be a float64 tensor")
@@ -170,22 +183,38 @@ def _apply_rinv(args: info, B: torch.Tensor, topo, trans: int, what: str) -> tor
     Xc = torch.empty_like(Bc)
     ctx = topo.context()
     cargs = args._c()
-    ctx.check(_lib.lib().capital_cholinv_apply_rinv_f64(ctx.handle, n, C.byref(cargs), _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
-                                                        args.R.data_ptr(), args.Rinv.data_ptr(), trans, k, Bc.data_ptr(), n,
-                                                        Xc.data_ptr(), n))
+    structure = _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT
+    if factor_r:
+        ctx.check(_lib.lib().capital_cholinv_apply_r_f64(ctx.handle, n, C.byref(cargs), structure, args.R.data_ptr(), trans, k,
+                                                         Bc.data_ptr(), n, Xc.data_ptr(), n))
+    else:
+        ctx.check(_lib.lib().capital_cholinv_apply_rinv_f64(ctx.handle, n, C.byref(cargs), structure, args.R.data_ptr(),
+                                                            args.Rinv.data_ptr(), trans, k, Bc.data_ptr(), n, Xc.data_ptr(), n))
     return Xc if B.dim() == 1 else Xc.t().contiguous()
 
 
 def apply_Rinv(args: info, B: torch.Tensor, topo) -> torch.Tensor:
     """X = R^-1 B from the factors of a previous `factor` (capital_cholinv_apply_rinv_f64, trans = 0): the back-transform x = R^-1 y of
     `sygst`.  B as for `solve`; returns X with B's shape and device, bit-identical on every rank."""
-    return _apply_rinv(args, B, topo, 0, "apply_Rinv")
+    return _apply(args, B, topo, 0, "apply_Rinv", False)
 
 
 def apply_RinvT(args: info, B: torch.Tensor, topo) -> torch.Tensor:
     """X = R^-T B (capital_cholinv_apply_rinv_f64, trans = 1): whitening.  apply_Rinv(args, apply_RinvT(args, B)) is solve(args, B),
     bit for bit."""
-    return _apply_rinv(args, B, topo, 1, "apply_RinvT")
+    return _apply(args, B, topo, 1, "apply_RinvT", False)
+
+
+def apply_R(args: info, Z: torch.Tensor, topo) -> torch.Tensor:
+    """X = R Z with the factor R of a previous `factor(B, args, topo)` (capital_cholinv_apply_r_f64, trans = 0); B Z = apply_RT(args,
+    apply_R(args, Z)).  Z as B for `solve`; returns X with Z's shape and device, bit-identical on every rank."""
+    return _apply(args, Z, topo, 0, "apply_R", True)
+
+
+def apply_RT(args: info, Z: torch.Tensor, topo) -> torch.Tensor:
+    """X = R^T Z (capital_cholinv_apply_r_f64, trans = 1): the back-transform x = R^T y of `sygst(..., itype=3)`, and samples of
+    covariance B from white noise Z."""
+    return _apply(args, Z, topo, 1, "apply_RT", True)
 
 
 def inverse_residual(A: matrix, Ainv: torch.Tensor, args: info, topo) -> float:

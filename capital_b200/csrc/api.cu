@@ -646,13 +646,16 @@ capital_status_t capital_cholinv_residual_f64(capital_ctx* ctx, const double* A_
 // node splits at s1): the block formula with R12 (the reference's cacqr::solve, cacqr.hpp:44-73)
 //   Y1 = Rinv11^T B1,  Y2 = Rinv22^T (B2 - R12^T Y1),  X2 = Rinv22 Y2,  X1 = Rinv11 (Y1 - R12 X2),
 // whose first three steps are Y = R^-T B and whose last three are X = R^-1 Y.  A half alone runs exactly the solve's steps of that half,
-// through the same panel intermediate T, so applying both halves in turn gives the solve's bits.
+// through the same panel intermediate T, so applying both halves in turn gives the solve's bits.  SOLVE_R / SOLVE_RT (X = R B, X = R^T B)
+// read only R: one pass over its triangle per panel, B copied into T first.
 static capital_status_t cholinv_solve_mode(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                            const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
                                            double* X, int64_t ldx, int mode, const char* what) {
-  if (!args || !Rinv_local || !B || !X || n <= 0 || nrhs < 1 || ldb < n || ldx < n || args->split <= 0 || args->dir != 'U' ||
-      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED)) {
-    ctx->set_error(std::string("cholinv::") + what + ": invalid arguments (Rinv, B, X non-null, nrhs >= 1, ldb, ldx >= n, split > 0 and dir == 'U')");
+  const bool apply_r = mode == SOLVE_R || mode == SOLVE_RT;
+  if (!args || (apply_r ? !R_local : !Rinv_local) || !B || !X || n <= 0 || nrhs < 1 || ldb < n || ldx < n || args->split <= 0 ||
+      args->dir != 'U' || (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED)) {
+    ctx->set_error(std::string("cholinv::") + what + ": invalid arguments (" + (apply_r ? "R" : "Rinv") +
+                   ", B, X non-null, nrhs >= 1, ldb, ldx >= n, split > 0 and dir == 'U')");
     return CAPITAL_ERR_INVALID;
   }
   CAP_CUDA(cudaSetDevice(ctx->device));
@@ -660,7 +663,7 @@ static capital_status_t cholinv_solve_mode(capital_ctx* ctx, int64_t n, const ca
   if (g.size > 1) return dist_cholinv_solve(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx, mode);
   const int64_t L = n;
   const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
-  const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
+  const bool skipped = !apply_r && args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
   if (skipped && !R_local) {
     ctx->set_error(std::string("cholinv::") + what + ": the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
     return CAPITAL_ERR_INVALID;
@@ -670,9 +673,9 @@ static capital_status_t cholinv_solve_mode(capital_ctx* ctx, int64_t n, const ca
   const size_t f_count = packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
   const int64_t ldu = packed ? 0 : L;
   cudaStream_t st = ctx->stream;
-  const double *dRi, *dR = nullptr, *dB;
-  CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
-  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
+  const double *dRi = nullptr, *dR = nullptr, *dB;
+  if (!apply_r) CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
+  if (skipped || apply_r) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
   CAP_TRY(cap_stage_in(ctx, B, (size_t)ldb * (nrhs - 1) + n, "solve_B", &dB));
   const bool x_host = !cap_is_device_ptr(X);
   double* dX = X;
@@ -700,6 +703,11 @@ static capital_status_t cholinv_solve_mode(capital_ctx* ctx, int64_t n, const ca
     const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
     const double* Bp = dB + p0 * ldb;
     double* Xp = dX + p0 * ldx;
+    if (apply_r) {
+      CAP_TRY(panel_add(ctx, st, L, w, Bp, ldb, nullptr, 0, T, L));
+      CAP_TRY(tri_apply(ctx, st, {dR, ldu, mode == SOLVE_RT, 0, L, 0, L, w, 1.0, T, 1, L, 0.0, nullptr, 0, Xp, 1, ldx}));  // R B, R^T B
+      continue;
+    }
     if (mode != SOLVE_RINV) CAP_TRY(half_t(Bp, w));
     else CAP_TRY(panel_add(ctx, st, L, w, Bp, ldb, nullptr, 0, T, L));
     if (mode != SOLVE_RINVT) CAP_TRY(half_n(Xp, w));
@@ -731,6 +739,18 @@ capital_status_t capital_cholinv_apply_rinv_f64(capital_ctx* ctx, int64_t n, con
   }
   return cholinv_solve_mode(ctx, n, args, structure, R_local, Rinv_local, nrhs, B, ldb, X, ldx, trans ? SOLVE_RINVT : SOLVE_RINV,
                             "apply_rinv");
+}
+
+// X = R B (trans = 0) or X = R^T B (trans = 1, the back-transform of sygst_ab for itype 3) with the factor's R.
+capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                             const double* R_local, int trans, int64_t nrhs, const double* B, int64_t ldb, double* X,
+                                             int64_t ldx) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (trans != 0 && trans != 1) {
+    ctx->set_error("cholinv::apply_r: trans must be 0 (X = R B) or 1 (X = R^T B)");
+    return CAPITAL_ERR_INVALID;
+  }
+  return cholinv_solve_mode(ctx, n, args, structure, R_local, nullptr, nrhs, B, ldb, X, ldx, trans ? SOLVE_RT : SOLVE_R, "apply_r");
 }
 
 // Do the byte ranges of a[0, na) and b[0, nb), two arrays of doubles, overlap?
@@ -866,6 +886,64 @@ capital_status_t capital_cholinv_sygst_f64(capital_ctx* ctx, int64_t n, const ca
   ops.A[0] = Ri; ops.B[0] = W;  // Rinv^T V
   ops.A[1] = W; ops.B[1] = Ri;  // V^T Rinv
   CAP_TRY(gemm_tn_x(ctx, st, L, L, L, 1.0, ops, 0.0, Cm, ld, CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER, 0, nullptr));
+  CAP_TRY(cap_stage_out_begin(ctx, C_local, count, "R_out", &dOut));
+  if (packed) CAP_TRY(pack_upper(ctx, st, L, Cm, ld, dOut, 0));
+  else CAP_TRY(sym_merge(ctx, st, L, Cm, ld, Cm, ld, true, dOut, L, 0, 0, 1));  // the lower half is the upper one's mirror, bit for bit
+  if (dOut != C_local) {
+    CAP_TRY(cap_stage_out_end(ctx, C_local, count, dOut));
+    CAP_CUDA(cudaStreamSynchronize(st));
+  }
+  return CAPITAL_OK;
+}
+
+// A B x = lambda x (itype 2) and B A x = lambda x (itype 3) with B = R^T R, both reduced to C y = lambda y with C = R A R^T (LAPACK
+// dsygst, itype 2 / 3, upper), in n^3 DMMA flops by the split of itype 1, A = U + U^T, C = M + M^T with M = R U R^T:
+//   W = R U = (R^T)^T U                        A_LOWER | B_UPPER | C_UPPER   n^3 / 3   (upper triangular: two upper factors)
+//   C_upper = (W^T)^T R^T + (R^T)^T W^T        A_LOWER | B_LOWER | C_UPPER   2 n^3 / 3, one launch with two operand classes
+// Only R is read, never Rinv, so a skipped top-level Rinv12 changes nothing.  U is the transpose of tril_half_copy's U^T, so only A's
+// lower triangle is read.  The only buffers are the factor's four workspaces: Ri = R, then U, then W^T; RiT = R^T; W = U^T, then W
+// (zeroed: the C_UPPER product leaves the strict lower part of its diagonal tiles unwritten, and W^T's diagonal tiles are read whole);
+// Rm = C.
+capital_status_t capital_cholinv_sygst_ab_f64(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                              const double* R_local, const double* A_local, double* C_local) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int64_t Lc = n > 0 ? ceil_div(n, std::max(ctx->grid.d, 1)) : 0;
+  const size_t count = packed ? (size_t)Lc * (Lc + 1) / 2 : (size_t)Lc * Lc, a_count = (size_t)Lc * Lc;
+  if (!args || !R_local || !A_local || !C_local || n <= 0 || args->split <= 0 || args->dir != 'U' ||
+      (structure != CAPITAL_RECT && structure != CAPITAL_UPPERTRI_PACKED) || overlaps(C_local, count, R_local, count) ||
+      overlaps(C_local, count, A_local, a_count)) {
+    ctx->set_error("cholinv::sygst_ab: invalid arguments (R, A and C non-null, C not overlapping A or R, split > 0 and dir == 'U', "
+                   "packed upper or rect)");
+    return CAPITAL_ERR_INVALID;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  const capital_grid_t& g = ctx->grid;
+  if (g.size > 1) return dist_cholinv_sygst_ab(ctx, n, args, structure, R_local, A_local, C_local);
+  const int64_t L = n, ld = round_up(L, 16);
+  cudaStream_t st = ctx->stream;
+  double *W, *Ri, *RiT, *Cm, *dOut;
+  CAP_TRY(ctx->workspace("W", (size_t)ld * L * 8, (void**)&W));
+  CAP_TRY(ctx->workspace("Ri", (size_t)ld * L * 8, (void**)&Ri));
+  CAP_TRY(ctx->workspace("RiT", (size_t)ld * L * 8, (void**)&RiT));
+  CAP_TRY(ctx->workspace("Rm", (size_t)ld * L * 8, (void**)&Cm));
+  // a host R is staged in the factor's R output buffer, which a host C reuses once R has been unpacked
+  const double *dR, *dA;
+  CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+  if (packed) CAP_TRY(unpack_upper(ctx, st, L, dR, Ri, ld));
+  else CAP_TRY(triu_copy(ctx, st, L, dR, L, Ri, ld, 0));
+  CAP_TRY(transpose_block(ctx, st, L, L, Ri, ld, RiT, ld, 1.0));  // R^T: lower, exact zeros above the diagonal
+  CAP_TRY(cap_stage_in(ctx, A_local, a_count, "A_in", &dA));
+  CAP_TRY(tril_half_copy(ctx, st, L, dA, L, W, ld, 0, 0, 1));      // U^T
+  CAP_TRY(transpose_block(ctx, st, L, L, W, ld, Ri, ld, 1.0));     // U
+  CAP_CUDA(cudaMemsetAsync(W, 0, (size_t)ld * L * 8, st));
+  CAP_TRY(gemm_tn(ctx, st, L, L, L, 1.0, RiT, ld, Ri, ld, 0.0, W, ld, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));
+  CAP_TRY(transpose_block(ctx, st, L, L, W, ld, Ri, ld, 1.0));     // W^T: lower, exact zeros above the diagonal
+  GemmOperands ops;
+  ops.ncls = 2; ops.lda = ops.ldb = ld;
+  ops.A[0] = Ri; ops.B[0] = RiT;  // W R^T
+  ops.A[1] = RiT; ops.B[1] = Ri;  // R W^T
+  CAP_TRY(gemm_tn_x(ctx, st, L, L, L, 1.0, ops, 0.0, Cm, ld, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER, 0, nullptr));
   CAP_TRY(cap_stage_out_begin(ctx, C_local, count, "R_out", &dOut));
   if (packed) CAP_TRY(pack_upper(ctx, st, L, Cm, ld, dOut, 0));
   else CAP_TRY(sym_merge(ctx, st, L, Cm, ld, Cm, ld, true, dOut, L, 0, 0, 1));  // the lower half is the upper one's mirror, bit for bit

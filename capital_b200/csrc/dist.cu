@@ -1215,6 +1215,10 @@ capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, 
 // exactly once.
 // A half alone (mode SOLVE_RINVT / SOLVE_RINV: capital_cholinv_apply_rinv_f64) runs that half's steps, with the same shares and the
 // same all-reduce slot set (signature cholsolve:n), so switching between solve and apply costs no arena clear.
+// SOLVE_R / SOLVE_RT (capital_cholinv_apply_r_f64) run one full-window step with R, again with those shares and slots.  The full window
+// includes the local diagonal, which on ranks with y > x lies below the global one: both output structures of the factor hold exact
+// zeros there (its base cases write them, and the packed and rect outputs copy them), as they do for Rinv, whose full window the solve
+// reads the same way.
 capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                     const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
                                     double* X, int64_t ldx, int mode) {
@@ -1224,7 +1228,8 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
   CAP_TRY(cholinv_shape(D, n, args));
   const capital_grid_t& g = D.g;
   const int64_t L = D.L, d = g.d;
-  const bool skipped = args->complete_inv == 0 && node_splits(D, L);  // the factor's predicate (cholinv_run)
+  const bool apply_r = mode == SOLVE_R || mode == SOLVE_RT;
+  const bool skipped = !apply_r && args->complete_inv == 0 && node_splits(D, L);  // the factor's predicate (cholinv_run)
   if (skipped && !R_local) {
     ctx->set_error("cholinv::solve: the top-level Rinv12 block was skipped (complete_inv = 0), R is needed");
     return CAPITAL_ERR_INVALID;
@@ -1234,9 +1239,9 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
   const size_t f_count = packed ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
   const int64_t ldu = packed ? 0 : L;
   cudaStream_t st = ctx->stream;
-  const double *dRi, *dR = nullptr, *dB;
-  CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
-  if (skipped) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
+  const double *dRi = nullptr, *dR = nullptr, *dB;
+  if (!apply_r) CAP_TRY(cap_stage_in(ctx, Rinv_local, f_count, "solve_Rinv", &dRi));
+  if (skipped || apply_r) CAP_TRY(cap_stage_in(ctx, R_local, f_count, "solve_R", &dR));
   CAP_TRY(cap_stage_in(ctx, B, (size_t)ldb * (nrhs - 1) + n, "solve_B", &dB));
   const bool x_host = !cap_is_device_ptr(X);
   double* dX = X;
@@ -1295,6 +1300,10 @@ capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_c
     const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
     const double* Bp = dB + p0 * ldb;
     double* Xp = dX + p0 * ldx;
+    if (apply_r) {  // X = R B or R^T B; the step writes Xp only after the all-reduce, so Xp may alias Bp
+      CAP_TRY(step(dR, mode == SOLVE_RT, 0, L, 0, L, w, 1.0, Bp, ldb, nullptr, 0, Xp, ldx));
+      continue;
+    }
     if (mode == SOLVE_RINV) {
       CAP_TRY(half_n(Bp, ldb, Xp, w));
       continue;
@@ -1552,6 +1561,110 @@ extern "C" capital_status_t capital_dist_trace_cholinv_sygst(const capital_grid_
     const bool skipped = args->complete_inv == 0 && node_splits(D, D.L);
     capital_status_t st = CAPITAL_OK;
     for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = sygst_run(D, v, skipped, CAPITAL_RECT, nullptr, nullptr, nullptr, nullptr);
+    return st;
+  });
+}
+
+// cholinv::sygst for itype 2 and 3 on the grid: C = R A R^T by the same split (api.cu, capital_cholinv_sygst_ab_f64), as three
+// distributed products with the depth reduction in the epilogue: W = (R^T)^T U, then C_upper = (W^T)^T R^T, then C_upper += (R^T)^T W^T
+// (beta = 1: the sum order is fixed).  R^T, U and W^T on rank (x, y, z) are the transposes of the partner (y, x, z)'s R, U^T and W
+// blocks (transpose_dist), as the inverse builds Rinv^T.  Globally R^T and W^T are lower triangular and U upper, and so are their local
+// blocks.  Only R is read: a skipped top-level Rinv12 changes nothing.  The rect output's lower half is the transpose partner's upper
+// half, merged in (sym_merge).  Every window of a mirror slot is pushed at most once per call.
+namespace {
+struct GstAB {
+  DMat R, RT, Au, U, W, WT, C, Ct;
+};
+// signature cholinv_gstab:L.  W's strict lower part is never written (C_UPPER product), so it keeps the zeros of the arena's clear,
+// which the partner's transpose turns into exact zeros above W^T's diagonal.
+size_t sygst_ab_layout(Dist& D, GstAB& v, char* base) {
+  Layout lay(base);
+  const int64_t L = D.L, ld = D.ld;
+  layout_mat(lay, D, v.R, ld, L, ROLE_T, false);           // T: the partner's R, for R^T
+  layout_mat(lay, D, v.RT, ld, L, ROLE_X | ROLE_Y, true);  // X: W's and the second term's R^T; Y: the first term's
+  layout_mat(lay, D, v.Au, ld, L, ROLE_T, false);          // U^T; T: the partner's, for U
+  layout_mat(lay, D, v.U, ld, L, ROLE_Y, false);
+  layout_mat(lay, D, v.W, ld, L, ROLE_T, false);           // T: the partner's W, for W^T
+  layout_mat(lay, D, v.WT, ld, L, ROLE_X | ROLE_Y, true);
+  layout_mat(lay, D, v.C, ld, L, ROLE_T, false);           // upper half of C; T: the partner's lower half of a rect output
+  layout_mat(lay, D, v.Ct, ld, L, 0, false);
+  layout_exchange(lay, D, Q_CHAIN, L, L);
+  return lay.off;
+}
+
+// dR, dA: the factor's R and A on the device; dOut: the local output block.  None is touched in a dry run.
+capital_status_t sygst_ab_run(Dist& D, GstAB& v, capital_structure_t structure, const double* dR, const double* dA, double* dOut) {
+  capital_ctx* ctx = D.ctx;
+  const capital_grid_t& g = D.g;
+  const int64_t L = D.L, ld = D.ld;
+  const int cs = S_CHAIN;
+  const bool packed = structure == CAPITAL_UPPERTRI_PACKED;
+  const int zdiag = g.y > g.x ? 1 : 0;  // there the local diagonal lies below the global one
+  ctx->comm_used = 0;
+  CAP_TRY(fork_streams(D));
+  if (!D.dry) CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), D.strm(cs)));
+  D.wr(cs, D.me, v.R.own, ld, L, L);
+  if (packed) DO(D, cs, unpack_upper(ctx, D.strm(cs), L, dR, v.R.own, ld));
+  else DO(D, cs, triu_copy(ctx, D.strm(cs), L, dR, L, v.R.own, ld, zdiag));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.R, 0, 0, L, L, ROLE_T, nullptr));
+  D.wr(cs, D.me, v.Au.own, ld, L, L);
+  DO(D, cs, tril_half_copy(ctx, D.strm(cs), L, dA, L, v.Au.own, ld, g.x, g.y, g.d));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.Au, 0, 0, L, L, ROLE_T, nullptr));
+  CAP_TRY(transpose_dist(D, Q_CHAIN, v.R, 0, 0, L, L, nullptr, v.RT.own, ld));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.RT, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
+  CAP_TRY(transpose_dist(D, Q_CHAIN, v.Au, 0, 0, L, L, nullptr, v.U.own, ld));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.U, 0, 0, L, L, ROLE_Y, nullptr));
+  const Win RT0{&v.RT, 0, 0}, WT0{&v.WT, 0, 0}, C0{&v.C, 0, 0};
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, RT0, Win{&v.U, 0, 0}, 0.0, Win{&v.W, 0, 0},
+                  CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER));  // W = R U
+  CAP_TRY(push(D, Q_CHAIN, cs, v.W, 0, 0, L, L, ROLE_T, nullptr));
+  CAP_TRY(transpose_dist(D, Q_CHAIN, v.W, 0, 0, L, L, nullptr, v.WT.own, ld));
+  CAP_TRY(push(D, Q_CHAIN, cs, v.WT, 0, 0, L, L, ROLE_X | ROLE_Y, nullptr));
+  const int tri = CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER;
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, WT0, RT0, 0.0, C0, tri));  // W R^T
+  CAP_TRY(product(D, Q_CHAIN, L, L, L, 1.0, RT0, WT0, 1.0, C0, tri));  // + R W^T
+  if (packed) {
+    D.rd(cs, v.C.own, ld, L, L);
+    DO(D, cs, pack_upper(ctx, D.strm(cs), L, v.C.own, ld, dOut, zdiag));
+  } else {
+    CAP_TRY(push(D, Q_CHAIN, cs, v.C, 0, 0, L, L, ROLE_T, nullptr));
+    CAP_TRY(transpose_dist(D, Q_CHAIN, v.C, 0, 0, L, L, nullptr, v.Ct.own, ld));
+    D.rd(cs, v.C.own, ld, L, L);
+    D.rd(cs, v.Ct.own, ld, L, L);
+    DO(D, cs, sym_merge(ctx, D.strm(cs), L, v.C.own, ld, v.Ct.own, ld, false, dOut, L, g.x, g.y, g.d));
+  }
+  return join_streams(D);
+}
+}  // namespace
+
+capital_status_t dist_cholinv_sygst_ab(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                       const double* R_local, const double* A_local, double* C_local) {
+  CAP_TRY(need_comm(ctx));
+  Dist D;
+  CAP_TRY(dist_setup(D, ctx, false));
+  CAP_TRY(cholinv_shape(D, n, args));
+  const int64_t L = D.L;
+  const size_t count = structure == CAPITAL_UPPERTRI_PACKED ? (size_t)L * (L + 1) / 2 : (size_t)L * L;
+  const double *dR, *dA;
+  double* dOut;
+  CAP_TRY(cap_stage_in(ctx, R_local, count, "R_out", &dR));
+  CAP_TRY(cap_stage_in(ctx, A_local, (size_t)L * L, "A_in", &dA));
+  CAP_TRY(cap_stage_out_begin(ctx, C_local, count, "gst_out", &dOut));
+  GstAB v;
+  CAP_TRY(arena_layout(ctx, "cholinv_gstab:" + std::to_string(L), [&](char* base) { return sygst_ab_layout(D, v, base); }));
+  CAP_TRY(sygst_ab_run(D, v, structure, dR, dA, dOut));
+  CAP_TRY(cap_stage_out_end(ctx, C_local, count, dOut));
+  return cap_check_info(ctx);
+}
+
+// Dry run of two consecutive capital_cholinv_sygst_ab_f64 calls (rect output) on one rank of a grid.
+extern "C" capital_status_t capital_dist_trace_cholinv_sygst_ab(const capital_grid_t* grid, int64_t n, const capital_cholinv_args_t* args,
+                                                                 int64_t* out, int64_t cap_records, int64_t* n_records) {
+  return dry_trace(grid, n, args, out, cap_records, n_records, [&](Dist& D, char* arena) {
+    GstAB v;
+    sygst_ab_layout(D, v, arena);
+    capital_status_t st = CAPITAL_OK;
+    for (int rep = 0; rep < 2 && st == CAPITAL_OK; rep++) st = sygst_ab_run(D, v, CAPITAL_RECT, nullptr, nullptr, nullptr);
     return st;
   });
 }

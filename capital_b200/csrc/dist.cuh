@@ -8,8 +8,9 @@ capital_status_t dist_cholinv_factor(capital_ctx* ctx, const double* A_local, in
                                      capital_structure_t ostruct, double* R_local, double* Rinv_local);
 capital_status_t dist_cholinv_residual(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
                                        const double* R_local, double* residual);
-// what the solve computes: A^-1 B (both halves), or one half alone: R^-1 B or R^-T B (capital_cholinv_apply_rinv_f64)
-enum { SOLVE_FULL = 0, SOLVE_RINV = 1, SOLVE_RINVT = 2 };
+// what the solve computes: A^-1 B (both halves), or one half alone: R^-1 B or R^-T B (capital_cholinv_apply_rinv_f64), or a product
+// with the factor itself: R B or R^T B (capital_cholinv_apply_r_f64)
+enum { SOLVE_FULL = 0, SOLVE_RINV = 1, SOLVE_RINVT = 2, SOLVE_R = 3, SOLVE_RT = 4 };
 capital_status_t dist_cholinv_solve(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                     const double* R_local, const double* Rinv_local, int64_t nrhs, const double* B, int64_t ldb,
                                     double* X, int64_t ldx, int mode);
@@ -17,6 +18,8 @@ capital_status_t dist_cholinv_inverse(capital_ctx* ctx, int64_t n, const capital
                                       const double* R_local, const double* Rinv_local, double* Ainv_local);
 capital_status_t dist_cholinv_sygst(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
                                     const double* R_local, const double* Rinv_local, const double* A_local, double* C_local);
+capital_status_t dist_cholinv_sygst_ab(capital_ctx* ctx, int64_t n, const capital_cholinv_args_t* args, capital_structure_t structure,
+                                       const double* R_local, const double* A_local, double* C_local);
 capital_status_t dist_cholinv_inverse_residual(capital_ctx* ctx, const double* A_local, int64_t n, capital_structure_t structure,
                                                const double* Ainv_local, double* residual);
 capital_status_t dist_cacqr_factor(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, int num_iter,

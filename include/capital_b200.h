@@ -141,6 +141,9 @@ capital_status_t capital_dist_trace_cholinv_inverse(const capital_grid_t* grid, 
 /* The same for two consecutive capital_cholinv_sygst_f64 calls (rect output) on a square grid. */
 capital_status_t capital_dist_trace_cholinv_sygst(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
                                                   int64_t* out, int64_t cap_records, int64_t* n_records);
+/* The same for two consecutive capital_cholinv_sygst_ab_f64 calls (rect output) on a square grid. */
+capital_status_t capital_dist_trace_cholinv_sygst_ab(const capital_grid_t* grid, int64_t n_global, const capital_cholinv_args_t* args,
+                                                     int64_t* out, int64_t cap_records, int64_t* n_records);
 
 /* ---- generators (device kernels; bit-exact with the reference's drand48-based ones) ---------- */
 /* matrix::distribute_symmetric(x, y, d, d, key, diagonallyDominant) -- structure.hpp:69-103. */
@@ -184,6 +187,15 @@ capital_status_t capital_cholinv_solve_f64(capital_ctx* ctx, int64_t n_global, c
 capital_status_t capital_cholinv_apply_rinv_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
                                                 capital_structure_t structure, const double* R_local, const double* Rinv_local,
                                                 int trans, int64_t nrhs, const double* B, int64_t ldb, double* X, int64_t ldx);
+/* A product with the factor itself: trans = 0: X = R B; trans = 1: X = R^T B (the back-transform x = R^T y of
+ * capital_cholinv_sygst_ab_f64 for B A x = lambda x; R^T xi draws samples of covariance B = R^T R from white noise xi).  Only R_local
+ * is read, exactly as the factor wrote it; Rinv is not an argument.  Otherwise arguments, conventions and guarantees as
+ * capital_cholinv_solve_f64: the full replicated B and X, X may alias B, bit-identical X on every rank, host or device pointers.  One
+ * pass over R's triangle per panel of up to 32 right-hand sides.  On a grid it uses the solve's all-reduce slots: switching between
+ * solve, apply_rinv and apply_r costs no arena clear. */
+capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                             capital_structure_t structure, const double* R_local, int trans, int64_t nrhs,
+                                             const double* B, int64_t ldb, double* X, int64_t ldx);
 
 /* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
  * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
@@ -212,6 +224,15 @@ capital_status_t capital_cholinv_inverse_f64(capital_ctx* ctx, int64_t n_global,
 capital_status_t capital_cholinv_sygst_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
                                            capital_structure_t structure, const double* R_local, const double* Rinv_local,
                                            const double* A_local, double* C_local);
+/* The other two generalized symmetric-definite eigenproblems, A B x = lambda x (LAPACK itype 2) and B A x = lambda x (itype 3), both
+ * reduced to standard form with the outputs of capital_cholinv_factor_f64 for B = R^T R (LAPACK dsygst, itype 2 / 3, upper):
+ * C = R A R^T, so that C y = lambda y and x = R^-1 y for itype 2 (capital_cholinv_apply_rinv_f64, trans = 0) or x = R^T y for itype 3
+ * (capital_cholinv_apply_r_f64, trans = 1).  Arguments and output as capital_cholinv_sygst_f64, except that only R is read (always
+ * complete, so complete_inv changes nothing) and Rinv is not an argument.  n^3 DMMA flops by the same split A = U + U^T: W = R U,
+ * then C = W R^T + R W^T, upper tiles only.  C must not overlap A or R.  CAPITAL_ERR_UNSUPPORTED when d does not divide n on a grid. */
+capital_status_t capital_cholinv_sygst_ab_f64(capital_ctx* ctx, int64_t n_global, const capital_cholinv_args_t* args,
+                                              capital_structure_t structure, const double* R_local, const double* A_local,
+                                              double* C_local);
 /* inverse::validate -- test/inverse/validate.hpp:7-34: ||A Ainv - I||_F / ||I||_F over the whole matrix, computed on the device(s),
  * the diagonal taken by GLOBAL index.  A_local: the full symmetric rect local block (as the generator writes it); Ainv_local: as
  * capital_cholinv_inverse_f64 wrote it in `structure`. */
