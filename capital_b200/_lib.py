@@ -17,7 +17,7 @@ EXPORTS = [  # every symbol include/capital_b200.h declares
     "capital_reset_counters", "capital_synchronize", "capital_set_stream", "capital_release_workspace", "capital_last_factor_ms", "capital_profile_begin", "capital_profile_end", "capital_probe_dmma_f64", "capital_blas_gemm_tn_tf32", "capital_set_trailing_precision", "capital_tf32_stats", "capital_timeline_begin", "capital_timeline_end", "capital_set_overlap", "capital_distribute_symmetric_f64",
     "capital_distribute_random_f64", "capital_cholinv_factor_f64", "capital_cholinv_residual_f64", "capital_cholinv_solve_f64",
     "capital_cholinv_inverse_f64", "capital_cholinv_inverse_residual_f64", "capital_cholinv_sygst_f64", "capital_cholinv_apply_rinv_f64",
-    "capital_cholinv_sygst_ab_f64", "capital_cholinv_apply_r_f64",
+    "capital_cholinv_sygst_ab_f64", "capital_cholinv_apply_r_f64", "capital_cholinv_factor_batched_f64", "capital_cholinv_solve_batched_f64",
     "capital_cacqr_factor_f64", "capital_cacqr_residual_f64", "capital_cacqr_apply_qt_f64", "capital_cacqr_apply_q_f64",
     "capital_cacqr_lstsq_f64", "capital_summa_gemm_tn_f64", "capital_blas_gemm_tn_f64",
     "capital_lapack_potrf_trtri_f64",
@@ -102,6 +102,8 @@ def lib() -> C.CDLL:
     L.capital_dist_trace_cholinv_sygst.argtypes = [C.POINTER(Grid), i64, C.POINTER(CholinvArgs), C.POINTER(i64), i64, C.POINTER(i64)]
     L.capital_cholinv_sygst_ab_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, vp, vp]
     L.capital_cholinv_apply_r_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, ci, i64, vp, i64, vp, i64]
+    L.capital_cholinv_factor_batched_f64.argtypes = [vp, i64, i64, vp, vp, vp, vp]
+    L.capital_cholinv_solve_batched_f64.argtypes = [vp, i64, i64, vp, i64, vp, vp]
     L.capital_dist_trace_cholinv_sygst_ab.argtypes = [C.POINTER(Grid), i64, C.POINTER(CholinvArgs), C.POINTER(i64), i64, C.POINTER(i64)]
     L.capital_cacqr_factor_f64.argtypes = [vp, vp, i64, i64, ci, C.POINTER(CholinvArgs), ci, vp, vp]
     L.capital_cacqr_residual_f64.argtypes = [vp, vp, i64, i64, vp, ci, vp, C.POINTER(dbl), C.POINTER(dbl)]

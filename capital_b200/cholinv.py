@@ -12,6 +12,8 @@
     C = cholinv.sygst(A2, args, topo, itype=2)                       # C = R A2 R^T for A2 A x = l x or A A2 x = l x (itype 3)
     X = cholinv.apply_R(args, Z, topo)                               # R Z (capital_cholinv_apply_r_f64)
     X = cholinv.apply_RT(args, Y, topo)                              # R^T Y, the itype 3 back-transform
+    R, Rinv, info = cholinv.factor_batched(A, topo)                  # many SPD matrices A[b] (n <= 512) at once
+    X = cholinv.solve_batched(Rinv, B, topo)                         # A[b] X[b] = B[b] from the batched factors
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -231,3 +233,66 @@ def inverse_residual(A: matrix, Ainv: torch.Tensor, args: info, topo) -> float:
                                                               _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT,
                                                               Ainv.data_ptr(), C.byref(r)))
     return float(r.value)
+
+
+_BATCHED_MAX_N = 512
+
+
+def _check_batched(t, what: str, name: str, ranks):
+    """ValueError unless t is a non-empty float64 tensor of one of the ranks in `ranks` (the device is checked by the caller, last)"""
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float64:
+        raise ValueError(f"cholinv.{what}: {name} must be a float64 tensor")
+    if t.dim() not in ranks or t.numel() == 0:
+        raise ValueError(f"cholinv.{what}: {name} has shape {tuple(t.shape)}")
+
+
+def factor_batched(A: torch.Tensor, topo):
+    """Factor a batch of SPD matrices at once (capital_cholinv_factor_batched_f64): A[b] = R[b].mT @ R[b] and Rinv[b] = R[b]^-1.
+    A: a CUDA float64 tensor of shape (b, n, n) with 1 <= n <= 512.  Only the LOWER triangle of each A[b] in torch indexing is read
+    (A[b, i, j] with i >= j, the diagonal included); A is never written.  Returns (R, Rinv, info): R and Rinv of shape (b, n, n), upper
+    triangular in torch indexing with exact zeros below the diagonal, and info, an int32 tensor of shape (b,): 0 where the factor
+    succeeded, else the 1-based pivot that was not positive.  A matrix that is not positive definite does not raise: check info, as
+    for torch.linalg.cholesky_ex.  Enqueued on the current stream without a host synchronisation.  On a grid, each rank factors its
+    own batch on its own GPU."""
+    _check_batched(A, "factor_batched", "A", (3,))
+    b, n = A.shape[0], A.shape[1]
+    if A.shape[2] != n:
+        raise ValueError(f"cholinv.factor_batched: A must have shape (b, n, n), got {tuple(A.shape)}")
+    if n > _BATCHED_MAX_N:
+        raise ValueError(f"cholinv.factor_batched: n = {n} > {_BATCHED_MAX_N} (factor such matrices one by one with cholinv.factor)")
+    if not A.is_cuda:
+        raise ValueError("cholinv.factor_batched: A must be a CUDA tensor")
+    # a row-major A[b] is the column-major A[b]^T: the upper triangle the library reads is A[b]'s lower triangle in torch indexing
+    Ac = A.contiguous()
+    Rc = torch.empty_like(Ac)
+    Ric = torch.empty_like(Ac)
+    info = torch.empty(b, dtype=torch.int32, device=A.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cholinv_factor_batched_f64(ctx.handle, n, b, Ac.data_ptr(), Rc.data_ptr(), Ric.data_ptr(),
+                                                            info.data_ptr()))
+    # column-major R[b] in a row-major buffer reads as R[b]^T: hand back the transposed views
+    return Rc.mT, Ric.mT, info
+
+
+def solve_batched(Rinv: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = A[b]^-1 B[b] with Rinv from `factor_batched` (capital_cholinv_solve_batched_f64): X = Rinv (Rinv^T B).  Rinv: CUDA float64
+    (b, n, n), upper triangular in torch indexing (only that triangle is read); B: CUDA float64 (b, n) or (b, n, k).  Returns X with B's
+    shape.  Enqueued on the current stream; deterministic."""
+    _check_batched(Rinv, "solve_batched", "Rinv", (3,))
+    _check_batched(B, "solve_batched", "B", (2, 3))
+    b, n = Rinv.shape[0], Rinv.shape[1]
+    if Rinv.shape[2] != n:
+        raise ValueError(f"cholinv.solve_batched: Rinv must have shape (b, n, n), got {tuple(Rinv.shape)}")
+    if n > _BATCHED_MAX_N:
+        raise ValueError(f"cholinv.solve_batched: n = {n} > {_BATCHED_MAX_N}")
+    if B.shape[0] != b or B.shape[1] != n:
+        raise ValueError(f"cholinv.solve_batched: B must have shape ({b}, {n}) or ({b}, {n}, k), got {tuple(B.shape)}")
+    if not Rinv.is_cuda or not B.is_cuda or Rinv.device != B.device:
+        raise ValueError("cholinv.solve_batched: Rinv and B must be CUDA tensors on the same device")
+    k = 1 if B.dim() == 2 else B.shape[2]
+    Uc = Rinv.mT.contiguous()                                # column-major Rinv[b] (no copy for factor_batched's output)
+    Bc = B.contiguous() if B.dim() == 2 else B.mT.contiguous()  # column-major n x k per matrix
+    Xc = torch.empty_like(Bc)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cholinv_solve_batched_f64(ctx.handle, n, b, Uc.data_ptr(), k, Bc.data_ptr(), Xc.data_ptr()))
+    return Xc if B.dim() == 2 else Xc.mT.contiguous()

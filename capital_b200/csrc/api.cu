@@ -753,6 +753,120 @@ capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n, const 
   return cholinv_solve_mode(ctx, n, args, structure, R_local, nullptr, nrhs, B, ldb, X, ldx, trans ? SOLVE_RT : SOLVE_R, "apply_r");
 }
 
+// ---- batched CholInv: many independent n x n matrices, n <= BASECASE_MAX, on this context's GPU ------------------------------------
+// Device memory the batched factor and solve hold for intermediates, whatever the batch: larger batches run in chunks.
+constexpr size_t BATCHED_WORKSPACE_CAP = size_t(2) << 30;
+
+// Cluster width of the batched cluster kernel for nb = 64 T: no phase of the kernel has work for more CTAs than tiles of a block row,
+// and an idle CTA still holds its SM's shared memory.  CAPITAL_BATCHED_CW=8 forces the single-matrix width (measurement).
+static int batched_cluster_width(int64_t nb) {
+  const char* e = getenv("CAPITAL_BATCHED_CW");
+  if (e && atoi(e) == 8) return 8;
+  const int64_t T = nb / 64;
+  return T <= 2 ? 2 : T <= 4 ? 4 : 8;
+}
+
+static bool all_device(std::initializer_list<const void*> ptrs) {
+  for (const void* p : ptrs)
+    if (!cap_is_device_ptr(p)) return false;
+  return true;
+}
+
+capital_status_t capital_cholinv_factor_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* A, double* R, double* Rinv,
+                                                    int* info) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!A || !R || !Rinv || !info || n < 1 || batch < 1) {
+    ctx->set_error("cholinv::factor_batched: invalid arguments (A, R, Rinv, info non-null, n >= 1, batch >= 1)");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error("cholinv::factor_batched: n > 512 is not supported (factor each matrix with capital_cholinv_factor_f64)");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device({A, R, Rinv, info})) {
+    ctx->set_error("cholinv::factor_batched: A, R, Rinv and info must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  const int64_t nn = n * n;
+  CAP_CUDA(cudaMemsetAsync(info, 0, (size_t)batch * sizeof(int), st));
+  if (n <= LEAF_MAX) {  // one CTA per matrix, straight from A's upper triangle into the outputs: no workspace
+    for (int64_t b0 = 0; b0 < batch; b0 += INT32_MAX) {
+      const LeafBatch bt{std::min<int64_t>(INT32_MAX, batch - b0), {nn, nn, nn, 0}, info + b0, 0};
+      CAP_TRY(leaf_cholinv(ctx, st, (int)n, A + b0 * nn, n, R + b0 * nn, n, Rinv + b0 * nn, n, nullptr, 0, &bt));
+    }
+    return CAPITAL_OK;
+  }
+  // the cluster kernel on nb = roundup(n, 64), identity pad; R and Rinv straight into the outputs when no pad is needed and they are
+  // 16-byte aligned (the kernel's 16-byte accesses; n is even then, so every matrix of the batch is aligned too)
+  const int64_t nb = round_up(n, 64), mm = nb * nb;
+  const bool direct = nb == n && (((uintptr_t)R | (uintptr_t)Rinv) & 15) == 0;
+  const int64_t chunk = std::min<int64_t>({batch, 65535, (int64_t)(BATCHED_WORKSPACE_CAP / ((direct ? 2 : 4) * mm * 8))});
+  double *W, *RiT, *Rw = nullptr, *Riw = nullptr;
+  CAP_TRY(ctx->workspace("batched_W", (size_t)(chunk * mm) * 8, (void**)&W));
+  CAP_TRY(ctx->workspace("batched_RiT", (size_t)(chunk * mm) * 8, (void**)&RiT));
+  if (!direct) {
+    CAP_TRY(ctx->workspace("batched_R", (size_t)(chunk * mm) * 8, (void**)&Rw));
+    CAP_TRY(ctx->workspace("batched_Ri", (size_t)(chunk * mm) * 8, (void**)&Riw));
+  }
+  const int cw = batched_cluster_width(nb);
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    CAP_TRY(sym_pad_batched(ctx, st, n, nb, cnt, A + b0 * nn, W));
+    if (direct) {
+      CAP_CUDA(cudaMemsetAsync(Rinv + b0 * nn, 0, (size_t)(cnt * nn) * 8, st));  // the kernel never writes Rinv's lower blocks
+      const LeafBatch bt{cnt, {mm, nn, nn, mm}, info + b0, cw};
+      CAP_TRY(basecase_cholinv(ctx, st, (int)nb, W, nb, R + b0 * nn, n, Rinv + b0 * nn, n, RiT, nb, &bt));
+    } else {
+      const LeafBatch bt{cnt, {mm, mm, mm, mm}, info + b0, cw};
+      CAP_TRY(basecase_cholinv(ctx, st, (int)nb, W, nb, Rw, nb, Riw, nb, RiT, nb, &bt));
+      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Rw, nb, mm, R + b0 * nn));
+      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Riw, nb, mm, Rinv + b0 * nn));
+    }
+  }
+  return CAPITAL_OK;
+}
+
+capital_status_t capital_cholinv_solve_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, int64_t nrhs,
+                                                   const double* B, double* X) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!Rinv || !B || !X || n < 1 || batch < 1 || nrhs < 1) {
+    ctx->set_error("cholinv::solve_batched: invalid arguments (Rinv, B, X non-null, n >= 1, batch >= 1, nrhs >= 1)");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error("cholinv::solve_batched: n > 512 is not supported");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device({Rinv, B, X})) {
+    ctx->set_error("cholinv::solve_batched: Rinv, B and X must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  const int64_t nn = n * n, nbk = n * nrhs, ts = n * SOLVE_W;
+  // per matrix: the panel intermediate T and tri_apply's partials (one k chunk per 64-row block: n <= 1024)
+  const int64_t per = (ts + round_up(n, 64) * SOLVE_W) * 8;
+  const int64_t chunk = std::min<int64_t>({batch, 65535, (int64_t)(BATCHED_WORKSPACE_CAP / per)});
+  double* T;
+  CAP_TRY(ctx->workspace("batched_T", (size_t)(chunk * ts) * 8, (void**)&T));
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    const double* U = Rinv + b0 * nn;
+    for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+      const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+      const double* Bp = B + b0 * nbk + p0 * n;
+      double* Xp = X + b0 * nbk + p0 * n;
+      // X may alias B: every matrix's panel of B is read into T before its panel of X is written
+      //                 U  ldu trans r0 r1 c0 c1 nrhs alpha P  pinc ldp beta Cin   ldcin C  cinc ldc full  batch su  sp   scin sc
+      CAP_TRY(tri_apply(ctx, st, {U, n, true, 0, n, 0, n, w, 1.0, Bp, 1, n, 0.0, nullptr, 0, T, 1, n, false, cnt, nn, nbk, 0, ts}));  // T = Rinv^T B
+      CAP_TRY(tri_apply(ctx, st, {U, n, false, 0, n, 0, n, w, 1.0, T, 1, n, 0.0, nullptr, 0, Xp, 1, n, false, cnt, nn, ts, 0, nbk}));  // X = Rinv T
+    }
+  }
+  return CAPITAL_OK;
+}
+
 // Do the byte ranges of a[0, na) and b[0, nb), two arrays of doubles, overlap?
 static bool overlaps(const double* a, size_t na, const double* b, size_t nb) {
   if (!a || !b) return false;

@@ -176,6 +176,12 @@ capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const d
 // (local (r, c) is global (y + d r, x + d c)) with its diagonal times 1/2, zeros above it.  The global upper triangle is never read.
 capital_status_t tril_half_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst, int64_t ldd,
                                 int x, int y, int d);
+// Batched factor (n <= BASECASE_MAX): W_b, nb x nb (nb a multiple of 32), from the upper triangle of A_b (n x n contiguous, mirrored below
+// the diagonal; the lower triangle is never read), the identity in the pad; and back: dst_b (n x n contiguous) = triu of the leading
+// n x n block of src_b (ld lds, stride ss), exact zeros below the diagonal.
+capital_status_t sym_pad_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t nb, int64_t batch, const double* A, double* W);
+capital_status_t triu_out_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
+                                  double* dst);
 capital_status_t gen_symmetric(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,
                                int64_t n_global, int x, int y, int d, int diag_dom);
 capital_status_t gen_random(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,
@@ -197,10 +203,19 @@ capital_status_t gram_shift_by(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
 // potrf('U') + trtri('U','N') of one nb x nb block (nb <= LEAF_MAX) in shared memory.
 constexpr int LEAF_MAX = 64;
 constexpr int BASECASE_MAX = 512;  // largest block handled by the one-launch cluster kernel (multiple of 64)
+// A batch of independent blocks in one launch: matrix b at W + b s.w, R + b s.r, ... with its own info[b], on clusters of cw CTAs
+// (2, 4 or 8; the cluster kernel only).  Without one (nullptr): a single block, ctx->d_info, width 8.
+struct BatchStrides { long long w = 0, r = 0, ri = 0, rit = 0; };
+struct LeafBatch {
+  int64_t batch;  // leaf: <= INT32_MAX; cluster kernel: <= 65535 (grid y)
+  BatchStrides s;
+  int* info;
+  int cw;
+};
 capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, double* W, int64_t ldw, double* R, int64_t ldr,
-                                  double* Ri, int64_t ldri, double* RiT, int64_t ldrit);
+                                  double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
 capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const double* W, int64_t ldw, double* R, int64_t ldr,
-                              double* Ri, int64_t ldri, double* RiT, int64_t ldrit);
+                              double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
 
 // ---- cholinv.cu -------------------------------------------------------------------------------
 // local (single-GPU) recursive CholInv on dense n x n blocks; W is destroyed (Schur complements).
@@ -246,6 +261,8 @@ struct TriApply {
   double* C;
   int64_t cinc, ldc;
   bool full = false;  // a rect window read whole (no j <= i mask, no triangular k ranges): Q^T P and Q P for a tall rect Q (ldu > 0)
+  // a batch of independent problems (<= 65535, grid z): matrix b reads U + b su, P + b sp, Cin + b scin and writes C + b sc
+  int64_t batch = 1, su = 0, sp = 0, scin = 0, sc = 0;
 };
 capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& a);
 // Y <- U[0:n, 0:n]^-1 Y in place for one panel of nrhs <= SOLVE_W right-hand sides (Y(k, w) at Y[k + w ldy]); U upper triangular,

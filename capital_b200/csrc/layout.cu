@@ -107,6 +107,40 @@ __global__ void tril_half_copy_kernel(long long n, const double* src, long long 
   }
 }
 
+// Copy-in of the batched factor: W_b (nb x nb, ld nb, at W + b nb nb) from the upper triangle of A_b (n x n, ld n, at A + b n n),
+// mirrored below the diagonal, and the identity in rows and columns n .. nb.  A's strictly lower triangle is never read.  The mirror
+// is a transposed read, staged in shared memory so that it stays coalesced; tiles wholly above the diagonal skip it.
+__global__ void sym_pad_batched_kernel(int n, int nb, const double* A, double* W) {
+  __shared__ double tile[TP][TP + 1];
+  const long long b = blockIdx.z;
+  A += b * n * n;
+  W += b * nb * nb;
+  const int r0 = blockIdx.x * TP, c0 = blockIdx.y * TP;
+  if (r0 + TP - 1 > c0) {
+    for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+      const int r = r0 + j, c = c0 + threadIdx.x;  // A(c, r), the mirror of element (r, c)
+      if (r < n && c < r) tile[j][threadIdx.x] = A[(long long)r * n + c];
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    double v = r == c ? 1.0 : 0.0;
+    if (r < n && c < n) v = r <= c ? A[(long long)c * n + r] : tile[threadIdx.x][j];
+    W[(long long)c * nb + r] = v;
+  }
+}
+
+// Copy-out of the batched factor: dst_b (n x n, ld n, at dst + b n n) = the upper triangle of the leading n x n block of src_b (ld lds,
+// at src + b ss), exact zeros below the diagonal.
+__global__ void triu_out_batched_kernel(long long n, long long batch, const double* src, long long lds, long long ss, double* dst) {
+  const long long nn = n * n, total = nn * batch;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / nn, e = i - b * nn, c = e / n, r = e - c * n;
+    dst[i] = r <= c ? src[b * ss + c * lds + r] : 0.0;
+  }
+}
+
 // drand48: X0 = seed<<16 | 0x330E ; X1 = (a X0 + c) mod 2^48 ; value = X1 / 2^48  (structure.hpp:80-85 re-seeds per element)
 __device__ __forceinline__ double drand48_first(unsigned long long seed) {
   const unsigned long long a = 0x5DEECE66DULL, c = 0xBULL, m48 = (1ULL << 48) - 1;
@@ -318,6 +352,21 @@ capital_status_t tril_half_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, co
                                 int x, int y, int d) {
   if (n <= 0) return CAPITAL_OK;
   tril_half_copy_kernel<<<(int)(n < ctx->num_sms * 8 ? n : ctx->num_sms * 8), 256, 0, st>>>(n, src, lds, dst, ldd, x, y, d);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t sym_pad_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t nb, int64_t batch, const double* A, double* W) {
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  if (nb < n || nb % TP != 0 || batch > 65535) return CAPITAL_ERR_INVALID;
+  dim3 grid((unsigned)(nb / TP), (unsigned)(nb / TP), (unsigned)batch), block(TP, 8);
+  sym_pad_batched_kernel<<<grid, block, 0, st>>>((int)n, (int)nb, A, W);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t triu_out_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
+                                  double* dst) {
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  triu_out_batched_kernel<<<grid_for(ctx, n * n * batch, 256), 256, 0, st>>>(n, batch, src, lds, ss, dst);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

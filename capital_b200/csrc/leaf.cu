@@ -4,11 +4,14 @@
 //
 // Two kernels share one device routine:
 //   leaf_kernel      one CTA, nb <= 64, everything in shared memory.
-//   basecase_kernel  one thread-block cluster (8 CTAs) for nb = 64 t (t <= 8): blocked right-looking Cholesky with
-//                    64-wide panels -- diagonal block by the leaf routine, row panel and trailing update as 64x64x64
+//   basecase_kernel  one thread-block cluster (CW = 2, 4 or 8 CTAs) for nb = 64 t (t <= 8): blocked right-looking Cholesky
+//                    with 64-wide panels -- diagonal block by the leaf routine, row panel and trailing update as 64x64x64
 //                    DMMA tile products spread over the cluster, hardware cluster barriers between phases -- followed
 //                    by the blocked triangular inverse.  One launch replaces ~60 latency-bound launches of the
 //                    recursion below 512, where leaves and small GEMMs are latency-bound.
+// Both take a batch of independent matrices (cholinv_factor_batched, api.cu): matrix b is blockIdx.x of the leaf kernel and
+// blockIdx.y of the cluster kernel (clusters stay along x), at per-matrix strides, with its own info[b].  The width CW only
+// decides which CTA computes which tile; every tile keeps its k range and k order, so a matrix gets the same bits at every width.
 // The critical path of a leaf is the pivot chain (64 dependent rsqrt + rank-1 updates), so the leaf keeps all
 // 256 threads on a fixed 16x16 grid (no index division), scales the pivot row with two warps, and uses one
 // rsqrt per pivot instead of a sqrt and a divide.
@@ -24,7 +27,6 @@ constexpr int LD = LEAF_MAX + 1;   // leaf arrays: conflict-free row and column 
 constexpr int TLD = 68;            // DMMA tiles: rows of 64 k-contiguous doubles, padded so that fragment loads
                                    // (row g, k q) of a half-warp touch 16 distinct bank pairs
 constexpr int TILE_DOUBLES = 64 * TLD;
-constexpr int BC_CLUSTER = 8;
 
 // 1/sqrt(d) off the critical path's slow library routine: FP32 seed + two FP64 Newton steps (relative error ~1e-16 for
 // d inside the FP32 range; outside it the library routine is used)
@@ -139,11 +141,14 @@ __device__ __forceinline__ void leaf_store(int nb, const double* a, const double
 
 __global__ void __launch_bounds__(256, 1)
     leaf_kernel(int nb, const double* W, long long ldw, double* __restrict__ R, long long ldr, double* __restrict__ Ri,
-                long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info) {
+                long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, BatchStrides bs) {
   extern __shared__ double sm[];
   double* a = sm;
   double* r = sm + LEAF_MAX * LD;
   double* t = sm + 2 * LEAF_MAX * LD;
+  const long long b = blockIdx.x;
+  W += b * bs.w; R += b * bs.r; Ri += b * bs.ri; info += b;
+  if (RiT != nullptr) RiT += b * bs.rit;
   leaf_load(nb, W, ldw, a);
   __syncthreads();
   leaf_factor_invert(nb, a, r, t, info, 0);
@@ -468,9 +473,15 @@ __device__ void leaf64_fast(double* __restrict__ sA, double* __restrict__ sR, do
 // W (nb x nb, upper read, destroyed) -> R, Ri, RiT blocks (full nb x nb blocks written: zeros in the other triangle).
 // Per block column jb:   [row panel over the cluster]  barrier  [trailing update over 7 CTAs  ||  the 8th: diagonal tile of
 // the next column first, then its leaf (lookahead)]  barrier.
-__global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
+template <int CW>
+__global__ void __cluster_dims__(CW, 1, 1) __launch_bounds__(256, 1)
     basecase_kernel(int nb, double* __restrict__ W, long long ldw, double* __restrict__ R, long long ldr, double* __restrict__ Ri,
-                    long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, long long* __restrict__ dbg) {
+                    long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, long long* __restrict__ dbg,
+                    BatchStrides bstr) {
+  {
+    const long long b = blockIdx.y;
+    W += b * bstr.w; R += b * bstr.r; Ri += b * bstr.ri; RiT += b * bstr.rit; info += b;
+  }
   extern __shared__ __align__(16) double sm[];
   double* sA = sm;                     // tile / leaf array a
   double* sB = sm + TILE_DOUBLES;      // tile / leaf array r
@@ -522,7 +533,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
     // row panel: R(jb, j) = Rinv_jj^T W(jb, j), j > jb
     int work = 0;
     for (int j = jb + 1; j < T; j++, work++) {
-      if (work % BC_CLUSTER != rank) continue;
+      if (work % CW != rank) continue;
       __syncthreads();
       tile_load(sA, Ri + o + o * ldri, ldri);                         // A[k][i] = Rinv_jj(k, i)
       tile_load(sB, W + o + (long long)j * 64 * ldw, ldw);            // B[k][c] = W(jb rows, j cols)
@@ -538,7 +549,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
     cluster.sync();
     if (jb == 0) DBG_STAMP();
     if (jb + 1 < T) {
-      const int leaf_rank = (jb + 1) % BC_CLUSTER;
+      const int leaf_rank = (jb + 1) % CW;
       if (rank == leaf_rank) {
         do_trailing(jb, jb + 1, jb + 1);   // lookahead: finish the next diagonal block first ...
         __threadfence_block();
@@ -549,7 +560,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
         for (int j = jb + 1; j < T; j++)
           for (int i = jb + 1; i <= j; i++) {
             if (i == jb + 1 && j == jb + 1) continue;
-            if (work++ % (BC_CLUSTER - 1) != slot) continue;
+            if (work++ % (CW - 1) != slot) continue;
             do_trailing(jb, i, j);
           }
       }
@@ -565,7 +576,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
     int work = 0;
     for (int j = 0; j < T; j++)
       for (int i = j + 1; i < T; i++, work++) {
-        if (work % BC_CLUSTER != rank) continue;
+        if (work % CW != rank) continue;
         for (int idx = threadIdx.x; idx < 4096; idx += 256)
           R[(long long)i * 64 + (idx & 63) + ((long long)j * 64 + (idx >> 6)) * ldr] = 0.0;
       }
@@ -583,7 +594,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
       const int jend = min(o + span, T);
       for (int j = o + bs; j < jend; j++)
         for (int i = o; i < o + bs; i++, work++) {
-          if (work % BC_CLUSTER != rank) continue;
+          if (work % CW != rank) continue;
           acc_zero(acc);
           for (int k = i; k < o + bs; k++) {
             __syncthreads();
@@ -607,7 +618,7 @@ __global__ void __cluster_dims__(BC_CLUSTER, 1, 1) __launch_bounds__(256, 1)
       const int jend = min(o + span, T);
       for (int j = o + bs; j < jend; j++)
         for (int i = o; i < o + bs; i++, work++) {
-          if (work % BC_CLUSTER != rank) continue;
+          if (work % CW != rank) continue;
           acc_zero(acc);
           for (int k = o + bs; k <= j; k++) {
             __syncthreads();
@@ -635,20 +646,23 @@ namespace {
 constexpr int LEAF_SMEM = 3 * LEAF_MAX * LD * (int)sizeof(double);
 constexpr int BASECASE_SMEM = (4 * TILE_DOUBLES + 128 + 512 + 256) * (int)sizeof(double);
 }  // namespace
-// per-device shared-memory opt-in of the two kernels (called from capital_create after cudaSetDevice)
+// per-device shared-memory opt-in of the kernels (called from capital_create after cudaSetDevice)
 capital_status_t leaf_init(capital_ctx* ctx) {
   CAP_CUDA(cudaFuncSetAttribute(leaf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, LEAF_SMEM));
-  CAP_CUDA(cudaFuncSetAttribute(basecase_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BASECASE_SMEM));
+  CAP_CUDA(cudaFuncSetAttribute(basecase_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, BASECASE_SMEM));
+  CAP_CUDA(cudaFuncSetAttribute(basecase_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, BASECASE_SMEM));
+  CAP_CUDA(cudaFuncSetAttribute(basecase_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, BASECASE_SMEM));
   return CAPITAL_OK;
 }
 
 capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const double* W, int64_t ldw, double* R, int64_t ldr, double* Ri,
-                              int64_t ldri, double* RiT, int64_t ldrit) {
+                              int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt) {
   if (nb <= 0) return CAPITAL_OK;
-  if (nb > LEAF_MAX) return CAPITAL_ERR_INVALID;
+  if (nb > LEAF_MAX || (bt && (bt->batch < 1 || bt->batch > INT32_MAX))) return CAPITAL_ERR_INVALID;
   constexpr int smem = LEAF_SMEM;
   const int tli = ctx->tl_begin(st, 4, nb);
-  leaf_kernel<<<1, 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, ctx->d_info);
+  leaf_kernel<<<bt ? (unsigned)bt->batch : 1u, 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, bt ? bt->info : ctx->d_info,
+                                                                bt ? bt->s : BatchStrides{});
   ctx->tl_end(st, tli);
   ctx->counters.kernel_launches++;
   ctx->counters.leaf_launches++;
@@ -658,16 +672,21 @@ capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const d
 
 // nb must be a multiple of 64, 128 <= nb <= BASECASE_MAX, and RiT non-null.
 capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, double* W, int64_t ldw, double* R, int64_t ldr, double* Ri,
-                                  int64_t ldri, double* RiT, int64_t ldrit) {
+                                  int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt) {
   if (nb % 64 != 0 || nb < 64 || nb > BASECASE_MAX || RiT == nullptr) return CAPITAL_ERR_INVALID;
+  const int cw = bt ? bt->cw : 8;
+  if (bt && (bt->batch < 1 || bt->batch > 65535)) return CAPITAL_ERR_INVALID;  // grid y
+  auto kernel = cw == 2 ? basecase_kernel<2> : cw == 4 ? basecase_kernel<4> : cw == 8 ? basecase_kernel<8> : nullptr;
+  if (!kernel) return CAPITAL_ERR_INVALID;
   constexpr int smem = BASECASE_SMEM;
   long long* dbg = nullptr;
-  if (getenv("CAPITAL_BC_DEBUG")) {
+  if (getenv("CAPITAL_BC_DEBUG") && !bt) {
     CAP_TRY(ctx->workspace("bc_dbg", 64 * sizeof(long long), (void**)&dbg));
     CAP_CUDA(cudaMemsetAsync(dbg, 0, 64 * sizeof(long long), st));
   }
   const int tli = ctx->tl_begin(st, 3, nb);
-  basecase_kernel<<<BC_CLUSTER, 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, ctx->d_info, dbg);
+  kernel<<<dim3(cw, bt ? (unsigned)bt->batch : 1u), 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, bt ? bt->info : ctx->d_info,
+                                                                      dbg, bt ? bt->s : BatchStrides{});
   ctx->tl_end(st, tli);
   if (dbg) {
     long long h[32];

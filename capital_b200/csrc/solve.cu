@@ -10,6 +10,9 @@
 // CTA each, longest blocks first; stage 1 writes one partial per chunk, stage 2 adds the chunks of a block in chunk order and
 // applies alpha, beta.  No atomics anywhere: the same inputs give the same bits (the grid solve relies on it).
 //
+// Batches (cholinv::solve_batched): blockIdx.z of stage 1 and the flat output index of stage 2 pick the matrix; U, P, the partials,
+// Cin and C advance by per-matrix strides.  Batch 1 is the single-matrix call, with the same arithmetic.
+//
 // FULL windows (cacqr::apply_QT / apply_Q / lstsq): the same kernel without the j <= i mask and with k over the whole other extent, so
 // a tall rect Q is read once for Q^T P (op T) or Q P (op N).  The substitution Y <- R^-1 Y of lstsq is tri_solve, at the end.
 #include "common.cuh"
@@ -31,6 +34,7 @@ struct TriDev {
   int64_t pinc, ldp;
   double* part;
   int64_t nob, cmax;
+  int64_t su, sp, spart;  // per-matrix strides (blockIdx.z)
 };
 
 // k range of owned block [olo, ohi): op T owns columns, k runs over the rows j <= i of the window; op N owns rows, k over the
@@ -47,7 +51,8 @@ __host__ __device__ inline int64_t n_chunks(int64_t klo, int64_t khi) {
   return (tiles + TA_KC - 1) / TA_KC;
 }
 
-template <int W, bool TRANS, bool FULL = false>
+// BATCH: blockIdx.z is the matrix (a separate instantiation, so that the single-matrix kernels keep their code and registers)
+template <int W, bool TRANS, bool FULL = false, bool BATCH = false>
 __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
   constexpr int WG = W >= 4 ? 4 : 1;  // w groups (each owns WPT right-hand sides)
   constexpr int KG = 4 / WG;           // k groups (narrow panels split k instead, summed in group order at the end)
@@ -79,7 +84,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
     const int64_t iend = TRANS ? ohi : khi;
     const bool row_ok = j < (TRANS ? khi : ohi);
     int64_t i = (TRANS ? olo : kb) + g;
-    const double* col = a.U + (packed ? i * (i + 1) / 2 : i * a.ldu);
+    const double* col = a.U + (BATCH ? blockIdx.z * a.su : 0) + (packed ? i * (i + 1) / 2 : i * a.ldu);
 #pragma unroll
     for (int it = 0; it < TA_PER; it++) {
       double v = 0.0;
@@ -94,7 +99,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
       const int kk = e & (TT - 1), w = e >> 6;
       const int64_t k = kb + kk;
       double v = 0.0;
-      if (e < TT * W && k < khi && w < a.nrhs) v = a.P[k * a.pinc + w * a.ldp];
+      if (e < TT * W && k < khi && w < a.nrhs) v = a.P[(BATCH ? blockIdx.z * a.sp : 0) + k * a.pinc + w * a.ldp];
       pr[p] = v;
     }
   };
@@ -151,7 +156,7 @@ __global__ void __launch_bounds__(TA_THREADS, 2) tri_apply_kernel(TriDev a) {
     }
   }
   if (kg == 0 && olo + oo < ohi) {
-    double* dst = a.part + ((b * a.cmax + blockIdx.x) * TT + oo) * W + wg * WPT;
+    double* dst = a.part + (BATCH ? blockIdx.z * a.spart : 0) + ((b * a.cmax + blockIdx.x) * TT + oo) * W + wg * WPT;
 #pragma unroll
     for (int q = 0; q < WPT; q++) dst[q] = acc[q];
   }
@@ -168,13 +173,18 @@ struct TriFin {
   int64_t ldcin;
   double* C;
   int64_t cinc, ldc;
+  int64_t batch, spart, scin, sc;  // matrices, per-matrix strides of part, Cin, C
 };
 
 // C(o, w) = alpha * (sum of the block's chunk partials, in chunk order) + beta * Cin(o, w)
 template <bool FULL = false>
 __global__ void tri_finish_kernel(TriFin f) {
-  const int64_t total = f.olen * f.nrhs;
-  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+  const int64_t per = f.olen * f.nrhs, total = per * f.batch;
+  for (int64_t gidx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; gidx < total; gidx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t mb = gidx / per, idx = gidx - mb * per;
+    const double* part = f.part + mb * f.spart;
+    const double* Cin = f.Cin ? f.Cin + mb * f.scin : nullptr;
+    double* C = f.C + mb * f.sc;
     const int64_t orel = idx % f.olen, w = idx / f.olen;
     const int64_t b = orel / TT, oo = orel % TT;
     const int64_t olo = f.o0 + b * TT, ohi = (f.o0 + f.olen) < olo + TT ? f.o0 + f.olen : olo + TT;
@@ -182,11 +192,11 @@ __global__ void tri_finish_kernel(TriFin f) {
     k_range<FULL>(f.trans, f.r0, f.r1, f.c0, f.c1, olo, ohi, &klo, &khi);
     const int64_t nch = n_chunks(klo, khi);
     double s = 0.0;
-    for (int64_t c = 0; c < nch; c++) s += f.part[((b * f.cmax + c) * TT + oo) * f.w + w];
+    for (int64_t c = 0; c < nch; c++) s += part[((b * f.cmax + c) * TT + oo) * f.w + w];
     const int64_t o = f.o0 + orel;
     double v = f.alpha * s;
-    if (f.Cin) v += f.beta * f.Cin[o * f.cinc + w * f.ldcin];
-    f.C[o * f.cinc + w * f.ldc] = v;
+    if (Cin) v += f.beta * Cin[o * f.cinc + w * f.ldcin];
+    C[o * f.cinc + w * f.ldc] = v;
   }
 }
 
@@ -195,46 +205,48 @@ __global__ void tri_finish_kernel(TriFin f) {
 // same bits for the same inputs
 __global__ void full_finish_kernel(TriFin f) {
   const int lane = threadIdx.x & 31;
-  const int64_t total = f.olen * f.nrhs;
+  const int64_t per = f.olen * f.nrhs, total = per * f.batch;
   int64_t klo, khi;
   k_range<true>(f.trans, f.r0, f.r1, f.c0, f.c1, 0, 0, &klo, &khi);
   const int64_t nch = n_chunks(klo, khi);
   const int64_t warps = (int64_t)gridDim.x * blockDim.x / 32;
-  for (int64_t idx = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32; idx < total; idx += warps) {
+  for (int64_t gidx = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) / 32; gidx < total; gidx += warps) {
+    const int64_t mb = gidx / per, idx = gidx - mb * per;
+    const double* part = f.part + mb * f.spart;
     const int64_t orel = idx % f.olen, w = idx / f.olen;
     const int64_t b = orel / TT, oo = orel % TT;
     double s = 0.0;
-    for (int64_t c = lane; c < nch; c += 32) s += f.part[((b * f.cmax + c) * TT + oo) * f.w + w];
+    for (int64_t c = lane; c < nch; c += 32) s += part[((b * f.cmax + c) * TT + oo) * f.w + w];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) {
       const int64_t o = f.o0 + orel;
       double v = f.alpha * s;
-      if (f.Cin) v += f.beta * f.Cin[o * f.cinc + w * f.ldcin];
-      f.C[o * f.cinc + w * f.ldc] = v;
+      if (f.Cin) v += f.beta * f.Cin[mb * f.scin + o * f.cinc + w * f.ldcin];
+      f.C[mb * f.sc + o * f.cinc + w * f.ldc] = v;
     }
   }
 }
 
-template <int W, bool TRANS, bool FULL>
+template <int W, bool TRANS, bool FULL, bool BATCH>
 capital_status_t launch_w(capital_ctx* ctx, cudaStream_t st, const TriDev& a, dim3 grid) {
   constexpr int PP = W == 1 ? 1 : W + 2;
   const size_t smem = (size_t)(TT * (TT + 1) + TT * PP) * 8;
-  CAP_CUDA(cudaFuncSetAttribute(tri_apply_kernel<W, TRANS, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  tri_apply_kernel<W, TRANS, FULL><<<grid, TA_THREADS, smem, st>>>(a);
+  CAP_CUDA(cudaFuncSetAttribute(tri_apply_kernel<W, TRANS, FULL, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  tri_apply_kernel<W, TRANS, FULL, BATCH><<<grid, TA_THREADS, smem, st>>>(a);
   CAP_CUDA(cudaGetLastError());
   return CAPITAL_OK;
 }
 
-template <bool TRANS, bool FULL>
+template <bool TRANS, bool FULL, bool BATCH = false>
 capital_status_t launch_op(capital_ctx* ctx, cudaStream_t st, int w, const TriDev& a, dim3 grid) {
   switch (w) {
-    case 1: return launch_w<1, TRANS, FULL>(ctx, st, a, grid);
-    case 2: return launch_w<2, TRANS, FULL>(ctx, st, a, grid);
-    case 4: return launch_w<4, TRANS, FULL>(ctx, st, a, grid);
-    case 8: return launch_w<8, TRANS, FULL>(ctx, st, a, grid);
-    case 16: return launch_w<16, TRANS, FULL>(ctx, st, a, grid);
-    default: return launch_w<32, TRANS, FULL>(ctx, st, a, grid);
+    case 1: return launch_w<1, TRANS, FULL, BATCH>(ctx, st, a, grid);
+    case 2: return launch_w<2, TRANS, FULL, BATCH>(ctx, st, a, grid);
+    case 4: return launch_w<4, TRANS, FULL, BATCH>(ctx, st, a, grid);
+    case 8: return launch_w<8, TRANS, FULL, BATCH>(ctx, st, a, grid);
+    case 16: return launch_w<16, TRANS, FULL, BATCH>(ctx, st, a, grid);
+    default: return launch_w<32, TRANS, FULL, BATCH>(ctx, st, a, grid);
   }
 }
 
@@ -245,6 +257,10 @@ constexpr int64_t TA_MAX_BLOCKS = 65535;  // owned blocks per launch (grid.y)
 capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x) {
   if (x.nrhs < 1 || x.nrhs > SOLVE_W) { ctx->set_error("tri_apply: 1 <= nrhs <= SOLVE_W"); return CAPITAL_ERR_INVALID; }
   if (x.full && x.ldu == 0) { ctx->set_error("tri_apply: a full window needs rect storage"); return CAPITAL_ERR_INVALID; }
+  if (x.batch < 1 || x.batch > TA_MAX_BLOCKS || (x.batch > 1 && x.full)) {
+    ctx->set_error("tri_apply: 1 <= batch <= 65535, and batches of triangular windows only");
+    return CAPITAL_ERR_INVALID;
+  }
   const int64_t o0 = x.trans ? x.c0 : x.r0, o1 = x.trans ? x.c1 : x.r1;
   if (o1 <= o0) return CAPITAL_OK;
   if (ceil_div(o1 - o0, TT) > TA_MAX_BLOCKS) {  // owned rows (columns) are independent: one launch per slab of them
@@ -270,15 +286,18 @@ capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x)
   }
   double* part = nullptr;
   if (cmax > 0) {
-    CAP_TRY(ctx->workspace("solve_part", (size_t)nob * cmax * TT * w * 8, (void**)&part));
-    TriDev a{x.U, x.ldu, x.r0, x.r1, x.c0, x.c1, (int)x.nrhs, x.P, x.pinc, x.ldp, part, nob, cmax};
-    const dim3 grid((unsigned)cmax, (unsigned)nob);
-    auto launch = x.full ? (x.trans ? launch_op<true, true> : launch_op<false, true>) : (x.trans ? launch_op<true, false> : launch_op<false, false>);
+    CAP_TRY(ctx->workspace("solve_part", (size_t)(nob * cmax * TT * w * x.batch) * 8, (void**)&part));
+    TriDev a{x.U, x.ldu, x.r0, x.r1, x.c0, x.c1, (int)x.nrhs, x.P, x.pinc, x.ldp, part, nob, cmax, x.su, x.sp, nob * cmax * TT * w};
+    const dim3 grid((unsigned)cmax, (unsigned)nob, (unsigned)x.batch);
+    auto launch = x.batch > 1 ? (x.trans ? launch_op<true, false, true> : launch_op<false, false, true>)
+                  : x.full    ? (x.trans ? launch_op<true, true> : launch_op<false, true>)
+                              : (x.trans ? launch_op<true, false> : launch_op<false, false>);
     CAP_TRY(launch(ctx, st, w, a, grid));
     ctx->counters.kernel_launches++;
   }
-  TriFin f{x.trans, x.r0, x.r1, x.c0, x.c1, o0, o1 - o0, (int)x.nrhs, w, part, cmax, x.alpha, x.beta, x.Cin, x.ldcin, x.C, x.cinc, x.ldc};
-  const int64_t total = (o1 - o0) * x.nrhs;
+  TriFin f{x.trans, x.r0, x.r1, x.c0, x.c1, o0, o1 - o0, (int)x.nrhs, w, part, cmax, x.alpha, x.beta, x.Cin, x.ldcin, x.C, x.cinc, x.ldc,
+           x.batch, nob * cmax * TT * w, x.scin, x.sc};
+  const int64_t total = (o1 - o0) * x.nrhs * x.batch;
   if (x.full && cmax > 32) {
     const int blocks = (int)std::min<int64_t>(ceil_div(total * 32, 256), 16 * (int64_t)ctx->num_sms);
     full_finish_kernel<<<blocks, 256, 0, st>>>(f);

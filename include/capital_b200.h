@@ -197,6 +197,25 @@ capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n_global,
                                              capital_structure_t structure, const double* R_local, int trans, int64_t nrhs,
                                              const double* B, int64_t ldb, double* X, int64_t ldx);
 
+/* Batched CholInv on this context's GPU: `batch` independent SPD matrices of order n <= 512, each factored A_b = R_b^T R_b with
+ * R_b^-1, in a few launches for the whole batch (one CTA per matrix for n <= 64, one thread-block cluster per matrix above).
+ * A, R, Rinv: batch x n x n, column-major, matrix b at offset b n n.  Only the upper triangle of each A_b, the diagonal included, is
+ * read; A is never written.  R_b and Rinv_b are written whole: upper triangular with exact zeros below the diagonal.  info[b] = 0 on
+ * success, else the 1-based pivot that was not positive (the factor then continues with 1 in its place, and the other matrices are
+ * unaffected); a non-SPD matrix is reported through info only, so the call returns CAPITAL_OK without waiting for the device.
+ * Device pointers only (CAPITAL_ERR_INVALID otherwise); R and Rinv must not overlap A.  Enqueued on the context stream; never
+ * communicates, so on a grid context each rank factors its own batch.  Intermediates take at most 2 GiB of device memory (kept
+ * until capital_release_workspace): larger batches run in chunks.  n > 512: CAPITAL_ERR_UNSUPPORTED; n < 1, batch < 1 or a NULL
+ * argument: CAPITAL_ERR_INVALID. */
+capital_status_t capital_cholinv_factor_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* A, double* R,
+                                                    double* Rinv, int* info);
+/* X_b = Rinv_b (Rinv_b^T B_b) = A_b^-1 B_b for the outputs of capital_cholinv_factor_batched_f64.  Rinv: batch x n x n as the factor
+ * wrote it (only its upper triangles are read); B, X: batch x n x nrhs, column-major, matrix b at offset b n nrhs.  X may alias B.
+ * Two passes over each Rinv_b per panel of up to 32 right-hand sides; deterministic.  Device pointers only; enqueued on the context
+ * stream.  Errors as capital_cholinv_factor_batched_f64 (nrhs < 1: CAPITAL_ERR_INVALID). */
+capital_status_t capital_cholinv_solve_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, int64_t nrhs,
+                                                   const double* B, double* X);
+
 /* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
  * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
  * local blocks exactly as the factor wrote them; R_local is read only when the top-level Rinv12 block was skipped (complete_inv = 0
