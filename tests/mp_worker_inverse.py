@@ -14,22 +14,7 @@ sys.path.insert(0, ROOT)
 import capital_b200 as cb
 from capital_b200 import _lib
 from oracle import capital_oracle as co
-
-
-def assemble(parts, coords, n, d, serialize):
-    """global matrix from the layer-0 local blocks: rect blocks as they are, packed ones through their (global) upper triangle"""
-    L = n // d
-    a = np.zeros((n, n))
-    for part, (x, y, z) in zip(parts, coords):
-        if z != 0:
-            continue
-        loc = co.unpack_upper(part, L) if serialize else part.reshape(L, L).T
-        gy, gx = np.meshgrid(y + d * np.arange(L), x + d * np.arange(L), indexing="ij")
-        keep = np.ones_like(loc, dtype=bool) if not serialize else gy <= gx
-        a[gy[keep], gx[keep]] = loc[keep]
-    if serialize:
-        a = np.triu(a) + np.triu(a, 1).T
-    return a
+from grid_edges_reference import assemble
 
 
 def main():

@@ -21,7 +21,7 @@ from capital_b200 import _lib
 from oracle import capital_oracle as co
 from sygst_ab_reference import bound, dsygst_full
 from sygst_reference import U
-from mp_worker_sygst import assemble
+from grid_edges_reference import assemble
 
 
 def main():
