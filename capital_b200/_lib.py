@@ -19,7 +19,7 @@ EXPORTS = [  # every symbol include/capital_b200.h declares
     "capital_cholinv_inverse_f64", "capital_cholinv_inverse_residual_f64", "capital_cholinv_sygst_f64", "capital_cholinv_apply_rinv_f64",
     "capital_cholinv_sygst_ab_f64", "capital_cholinv_apply_r_f64", "capital_cholinv_factor_batched_f64", "capital_cholinv_solve_batched_f64",
     "capital_cacqr_factor_f64", "capital_cacqr_residual_f64", "capital_cacqr_apply_qt_f64", "capital_cacqr_apply_q_f64",
-    "capital_cacqr_lstsq_f64", "capital_summa_gemm_tn_f64", "capital_blas_gemm_tn_f64",
+    "capital_cacqr_lstsq_f64", "capital_cacqr_factor_batched_f64", "capital_cacqr_lstsq_batched_f64", "capital_summa_gemm_tn_f64", "capital_blas_gemm_tn_f64",
     "capital_lapack_potrf_trtri_f64",
 ]
 
@@ -110,6 +110,8 @@ def lib() -> C.CDLL:
     L.capital_cacqr_apply_qt_f64.argtypes = [vp, i64, i64, vp, i64, vp, i64, vp, i64]
     L.capital_cacqr_apply_q_f64.argtypes = [vp, i64, i64, vp, i64, vp, i64, vp, i64]
     L.capital_cacqr_lstsq_f64.argtypes = [vp, i64, i64, vp, ci, vp, i64, vp, i64, vp, i64]
+    L.capital_cacqr_factor_batched_f64.argtypes = [vp, i64, i64, i64, ci, vp, vp, vp, vp]
+    L.capital_cacqr_lstsq_batched_f64.argtypes = [vp, i64, i64, i64, vp, vp, i64, vp, vp]
     L.capital_summa_gemm_tn_f64.argtypes = [vp, i64, i64, i64, dbl, vp, vp, dbl, vp]
     L.capital_blas_gemm_tn_f64.argtypes = [vp, i64, i64, i64, dbl, vp, i64, vp, i64, dbl, vp, i64, ci]
     L.capital_lapack_potrf_trtri_f64.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64]

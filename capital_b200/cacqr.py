@@ -6,6 +6,8 @@
     Y = cacqr.apply_QT(B, args, topo)               # cacqr.h:55: Q^T B      (capital_cacqr_apply_qt_f64)
     C = cacqr.apply_Q(Z, args, topo)                # cacqr.h:52: Q Z        (capital_cacqr_apply_q_f64)
     X = cacqr.lstsq(args, B, topo)                  # argmin ||A X - B|| = R^-1 Q^T B   (capital_cacqr_lstsq_f64)
+    Q, R, info = cacqr.factor_batched(A, topo, 2)   # many (b, m, n) matrices, n <= 512, one GPU (capital_cacqr_factor_batched_f64)
+    X = cacqr.lstsq_batched(Q, R, B, topo)          # X[b] = R[b]^-1 Q[b]^T B[b]  (capital_cacqr_lstsq_batched_f64)
 
 num_iter = 3 is shifted CholeskyQR3 (Fukaya et al., SIAM J. Sci. Comput. 42(1), 2020), an extension beyond the reference: a first
 sweep on the shifted Gram matrix G + s I, s = 11 (m n + n (n + 1)) 2^-53 trace(G), then CholeskyQR2 on its Q; R = R3 R2 R1.  It
@@ -136,3 +138,76 @@ def lstsq(args: info, B: torch.Tensor, topo) -> torch.Tensor:
                                                  _lib.UPPERTRI_PACKED if args.serialize else _lib.RECT, args.R.data_ptr(), k,
                                                  Bc.data_ptr(), args.rows_local, Xc.data_ptr(), n))
     return _result(Xc, B.dim())
+
+
+_BATCHED_MAX_N = 512
+
+
+def _check_batched(t, what: str, name: str, ranks):
+    """ValueError unless t is a non-empty float64 tensor of one of the ranks in `ranks` (the device is checked by the caller, last)"""
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.float64:
+        raise ValueError(f"cacqr.{what}: {name} must be a float64 tensor")
+    if t.dim() not in ranks or t.numel() == 0:
+        raise ValueError(f"cacqr.{what}: {name} has shape {tuple(t.shape)}")
+
+
+def _colmajor_batch(T: torch.Tensor) -> torch.Tensor:
+    """the (b, cols, rows) buffer whose matrices are T[b] column-major: T.mT itself when it is contiguous, else one copy"""
+    Tt = T.mT
+    return Tt if Tt.is_contiguous() else Tt.contiguous()
+
+
+def factor_batched(A: torch.Tensor, topo, num_iter: int = 2):
+    """QR of a batch of tall-skinny matrices at once (capital_cacqr_factor_batched_f64): A[b] = Q[b] @ R[b].  A: a CUDA float64
+    tensor of shape (b, m, n) with 1 <= n <= 512 and m >= n; when A.mT is contiguous (A[b] column-major) it is read without a copy.
+    num_iter: 1 = CholeskyQR, 2 = CholeskyQR2, 3 = shifted CholeskyQR3 (as in cacqr.info).  Returns (Q, R, info): Q of shape
+    (b, m, n), R of shape (b, n, n), upper triangular with exact zeros below the diagonal (both .mT views of column-major buffers),
+    and info, an int32 tensor of shape (b,): 0 where the factor succeeded, else the 1-based pivot of the first sweep whose Gram
+    matrix was not positive definite (Q[b] and R[b] are then unspecified).  A failure does not raise: check info.  Enqueued on the
+    current stream without a host synchronisation.  On a grid, each rank factors its own batch on its own GPU."""
+    _check_batched(A, "factor_batched", "A", (3,))
+    b, m, n = A.shape
+    if int(num_iter) not in (1, 2, 3):
+        raise ValueError(f"cacqr.factor_batched: num_iter must be 1, 2 or 3, got {num_iter}")
+    if n > _BATCHED_MAX_N:
+        raise ValueError(f"cacqr.factor_batched: n = {n} > {_BATCHED_MAX_N} (factor such matrices one by one with cacqr.factor)")
+    if m < n:
+        raise ValueError(f"cacqr.factor_batched: m = {m} < n = {n}")
+    if not A.is_cuda:
+        raise ValueError("cacqr.factor_batched: A must be a CUDA tensor")
+    Ac = _colmajor_batch(A)
+    Qc = torch.empty((b, n, m), dtype=torch.float64, device=A.device)
+    Rc = torch.empty((b, n, n), dtype=torch.float64, device=A.device)
+    info = torch.empty(b, dtype=torch.int32, device=A.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cacqr_factor_batched_f64(ctx.handle, m, n, b, int(num_iter), Ac.data_ptr(), Qc.data_ptr(),
+                                                          Rc.data_ptr(), info.data_ptr()))
+    return Qc.mT, Rc.mT, info
+
+
+def lstsq_batched(Q: torch.Tensor, R: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = R[b]^-1 Q[b]^T B[b] = argmin ||A[b] X - B[b]|| from the outputs of `factor_batched` (capital_cacqr_lstsq_batched_f64).
+    Q: CUDA float64 (b, m, n); R: CUDA float64 (b, n, n), upper triangular (only that triangle is read); B: CUDA float64 (b, m) or
+    (b, m, k).  Returns X of shape (b, n) or (b, n, k).  Enqueued on the current stream; deterministic."""
+    _check_batched(Q, "lstsq_batched", "Q", (3,))
+    _check_batched(R, "lstsq_batched", "R", (3,))
+    _check_batched(B, "lstsq_batched", "B", (2, 3))
+    b, m, n = Q.shape
+    if R.shape != (b, n, n):
+        raise ValueError(f"cacqr.lstsq_batched: R must have shape ({b}, {n}, {n}), got {tuple(R.shape)}")
+    if n > _BATCHED_MAX_N:
+        raise ValueError(f"cacqr.lstsq_batched: n = {n} > {_BATCHED_MAX_N}")
+    if m < n:
+        raise ValueError(f"cacqr.lstsq_batched: m = {m} < n = {n}")
+    if B.shape[0] != b or B.shape[1] != m:
+        raise ValueError(f"cacqr.lstsq_batched: B must have shape ({b}, {m}) or ({b}, {m}, k), got {tuple(B.shape)}")
+    if not Q.is_cuda or not R.is_cuda or not B.is_cuda or len({Q.device, R.device, B.device}) != 1:
+        raise ValueError("cacqr.lstsq_batched: Q, R and B must be CUDA tensors on the same device")
+    k = 1 if B.dim() == 2 else B.shape[2]
+    Qc, Rc = _colmajor_batch(Q), _colmajor_batch(R)
+    Bc = B.contiguous() if B.dim() == 2 else _colmajor_batch(B)
+    Xc = torch.empty((b, n) if B.dim() == 2 else (b, k, n), dtype=torch.float64, device=B.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cacqr_lstsq_batched_f64(ctx.handle, m, n, b, Qc.data_ptr(), Rc.data_ptr(), k, Bc.data_ptr(),
+                                                         Xc.data_ptr()))
+    return Xc if B.dim() == 2 else Xc.mT

@@ -757,15 +757,6 @@ capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n, const 
 // Device memory the batched factor and solve hold for intermediates, whatever the batch: larger batches run in chunks.
 constexpr size_t BATCHED_WORKSPACE_CAP = size_t(2) << 30;
 
-// Cluster width of the batched cluster kernel for nb = 64 T: no phase of the kernel has work for more CTAs than tiles of a block row,
-// and an idle CTA still holds its SM's shared memory.  CAPITAL_BATCHED_CW=8 forces the single-matrix width (measurement).
-static int batched_cluster_width(int64_t nb) {
-  const char* e = getenv("CAPITAL_BATCHED_CW");
-  if (e && atoi(e) == 8) return 8;
-  const int64_t T = nb / 64;
-  return T <= 2 ? 2 : T <= 4 ? 4 : 8;
-}
-
 static bool all_device(std::initializer_list<const void*> ptrs) {
   for (const void* p : ptrs)
     if (!cap_is_device_ptr(p)) return false;
@@ -1161,6 +1152,53 @@ capital_status_t capital_cacqr_lstsq_f64(capital_ctx* ctx, int64_t m, int64_t n,
   }
   CAP_CUDA(cudaSetDevice(ctx->device));
   return dist_cacqr_apply_qt(ctx, m, n, Q_local, rstruct, R_local, nrhs, B_local, ldb, X, ldx);
+}
+
+// ---- batched CholeskyQR: many independent m x n matrices, n <= BASECASE_MAX, on this context's GPU (dist.cu) ----------------------
+capital_status_t capital_cacqr_factor_batched_f64(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, int num_iter, const double* A,
+                                                  double* Q, double* R, int* info) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!A || !Q || !R || !info || n < 1 || m < n || batch < 1 || num_iter < 1 || num_iter > 3) {
+    ctx->set_error("cacqr::factor_batched: invalid arguments (A, Q, R, info non-null, m >= n >= 1, batch >= 1, num_iter 1, 2 or 3)");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error("cacqr::factor_batched: n > 512 is not supported (factor each matrix with capital_cacqr_factor_f64)");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device({A, Q, R, info})) {
+    ctx->set_error("cacqr::factor_batched: A, Q, R and info must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (overlaps(A, (size_t)(batch * m * n), Q, (size_t)(batch * m * n))) {
+    ctx->set_error("cacqr::factor_batched: Q must not overlap A");
+    return CAPITAL_ERR_INVALID;
+  }
+  return dist_cacqr_factor_batched(ctx, m, n, batch, num_iter, A, Q, R, info);
+}
+
+capital_status_t capital_cacqr_lstsq_batched_f64(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, const double* Q, const double* R,
+                                                 int64_t nrhs, const double* B, double* X) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!Q || !R || !B || !X || n < 1 || m < n || batch < 1 || nrhs < 1) {
+    ctx->set_error("cacqr::lstsq_batched: invalid arguments (Q, R, B, X non-null, m >= n >= 1, batch >= 1, nrhs >= 1)");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error("cacqr::lstsq_batched: n > 512 is not supported");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device({Q, R, B, X})) {
+    ctx->set_error("cacqr::lstsq_batched: Q, R, B and X must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (overlaps(B, (size_t)(batch * m * nrhs), X, (size_t)(batch * n * nrhs))) {
+    ctx->set_error("cacqr::lstsq_batched: X must not overlap B");
+    return CAPITAL_ERR_INVALID;
+  }
+  return dist_cacqr_lstsq_batched(ctx, m, n, batch, Q, R, nrhs, B, X);
 }
 
 // ---- SUMMA -----------------------------------------------------------------------------------

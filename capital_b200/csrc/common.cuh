@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <string>
 #include <vector>
@@ -146,6 +147,20 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags);
 capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const double* A, int64_t lda,
                            const double* B, int64_t ldb, double* C, int64_t ldc, double* Ct, int64_t ldct, int flags);
+// split-k chunk count of gemm_tn_splitk for this shape (and whether it runs 128 x 128 tiles)
+int64_t gemm_splitk_chunks(const capital_ctx* ctx, int64_t m, int64_t n, int64_t k, int flags, bool* big);
+// A batch of products of one shape: matrix b reads A + b sa and B + b sb (16-byte aligned bases, even lda, ldb, sa, sb) and writes
+// C + b sc, Ct + b sct (gemm_tn_batched, gemm_tn.cu)
+struct GemmBatchOps {
+  int64_t batch = 1;
+  const double* A = nullptr;
+  int64_t lda = 0, sa = 0;
+  const double* B = nullptr;
+  int64_t ldb = 0, sb = 0;
+  int64_t sc = 0, sct = 0;
+};
+capital_status_t gemm_tn_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmBatchOps& b,
+                                 double* C, int64_t ldc, double* Ct, int64_t ldct, int flags, bool gram);
 
 // ---- gemm_tf32.cu (experimental mixed-precision trailing update, BASELINE config 5) ----------------------------
 capital_status_t gemm_tf32_init(capital_ctx* ctx);
@@ -198,6 +213,12 @@ capital_status_t gram_shift(capital_ctx* ctx, cudaStream_t st, int64_t n, double
 capital_status_t gram_diag_partial(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* G, int64_t ld, double* out);
 capital_status_t gram_shift_by(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, const double* parts, int nparts,
                                double coef);
+// Batches (<= 65535 matrices, matrix b at src + b ss, dst + b sd): gram_shift with one CTA per matrix, in gram_shift's summation order;
+// and transpose_block (scale 1) of every matrix.
+capital_status_t gram_shift_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, double* G, int64_t ld, int64_t sg,
+                                    double coef);
+capital_status_t transpose_batched(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, int64_t batch, const double* src,
+                                   int64_t lds, int64_t ss, double* dst, int64_t ldd, int64_t sd);
 
 // ---- leaf.cu ----------------------------------------------------------------------------------
 // potrf('U') + trtri('U','N') of one nb x nb block (nb <= LEAF_MAX) in shared memory.
@@ -216,6 +237,14 @@ capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, dou
                                   double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
 capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const double* W, int64_t ldw, double* R, int64_t ldr,
                               double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
+// Cluster width of the batched cluster kernel for nb = 64 T: no phase of the kernel has work for more CTAs than tiles of a block row,
+// and an idle CTA still holds its SM's shared memory.  CAPITAL_BATCHED_CW=8 forces the single-matrix width (measurement).
+static inline int batched_cluster_width(int64_t nb) {
+  const char* e = getenv("CAPITAL_BATCHED_CW");
+  if (e && atoi(e) == 8) return 8;
+  const int64_t T = nb / 64;
+  return T <= 2 ? 2 : T <= 4 ? 4 : 8;
+}
 
 // ---- cholinv.cu -------------------------------------------------------------------------------
 // local (single-GPU) recursive CholInv on dense n x n blocks; W is destroyed (Schur complements).
@@ -269,6 +298,9 @@ capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& a)
 // packed (ldu == 0) or rect, entries below the diagonal never read.  Deterministic.
 capital_status_t tri_solve(capital_ctx* ctx, cudaStream_t st, const double* U, int64_t ldu, int64_t n, int64_t nrhs, double* Y,
                            int64_t ldy);
+// tri_solve on a batch of <= 65535 independent problems: U + b su (rect), Y + b sy; each gets tri_solve's bits
+capital_status_t tri_solve_batched(capital_ctx* ctx, cudaStream_t st, const double* U, int64_t ldu, int64_t su, int64_t n, int64_t nrhs,
+                                   double* Y, int64_t ldy, int64_t sy, int64_t batch);
 // Out = S + Cin (Cin may be null) on a rows x w column-major panel
 capital_status_t panel_add(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t w, const double* S, int64_t lds, const double* Cin,
                            int64_t ldcin, double* Out, int64_t ldo);

@@ -2412,3 +2412,156 @@ capital_status_t dist_cacqr_apply_q(capital_ctx* ctx, int64_t m, int64_t n, cons
   }
   return CAPITAL_OK;
 }
+
+// ---- batched CholeskyQR2: many independent m x n matrices, n <= BASECASE_MAX, on this context's GPU -------------------------------
+// Each step of sweep() above, batched: the split-k Gram product with gemm_tn_splitk's chunk rule, the Gram shift, the batched base case
+// of cholinv::factor_batched, the apply Q <- Q Rinv as Rinv^T Q^T with Q's transposed store, and R = R2 R1 (R3 (R2 R1)).  Every product
+// keeps the single path's k range and order, so where the single path's base case is one kernel (n <= 64 or n a multiple of 64) a
+// matrix gets the single path's bits.  Matrix b of A and Q is at b m n (ld m), of R at b n n (ld n); intermediates use the single
+// path's leading dimensions.
+namespace {
+// Device memory the batched CholeskyQR holds for intermediates, whatever the batch (BATCHED_WORKSPACE_CAP of the batched CholInv)
+constexpr int64_t QR_BATCHED_CAP = int64_t(2) << 30;
+
+struct QrB {
+  capital_ctx* ctx;
+  cudaStream_t st;
+  int64_t m, n, cnt;
+  int64_t ldq, ldt, nr, nb;  // panel copies, transposed panels, n x n factors, padded base-case block
+  double *Q, *Qt, *Qt2, *G, *W, *RiT, *Ri;
+  int* info;
+};
+
+// sweep() for every matrix of the chunk: Qc (ldqc, stride sqc) -> Gram; QtIn (ld ldt, stride ldt m) -> the apply, whose plain store
+// writes QtOut (optional) and whose transposed store writes QcOut (ldqo, stride sqo); R lands in Rout (nr x nr per matrix)
+capital_status_t sweep_batched(QrB& q, const double* Qc, int64_t ldqc, int64_t sqc, const double* QtIn, double* QtOut, double* QcOut,
+                               int64_t ldqo, int64_t sqo, double* Rout, double shift = 0.0) {
+  capital_ctx* ctx = q.ctx;
+  cudaStream_t st = q.st;
+  const int64_t n = q.n, m = q.m, cnt = q.cnt, rr = q.nr * q.nr;
+  GemmBatchOps g;
+  g.batch = cnt; g.A = Qc; g.lda = ldqc; g.sa = sqc; g.B = Qc; g.ldb = ldqc; g.sb = sqc; g.sc = n * n;
+  CAP_TRY(gemm_tn_batched(ctx, st, n, n, m, 1.0, g, q.G, n, nullptr, 0, CAPITAL_GEMM_C_UPPER, true));
+  if (shift > 0.0) CAP_TRY(gram_shift_batched(ctx, st, n, cnt, q.G, n, n * n, shift));
+  CAP_CUDA(cudaMemsetAsync(q.Ri, 0, (size_t)(cnt * rr) * 8, st));
+  CAP_CUDA(cudaMemsetAsync(Rout, 0, (size_t)(cnt * rr) * 8, st));
+  if (n <= LEAF_MAX) {
+    const LeafBatch bt{cnt, {n * n, rr, rr, 0}, q.info, 0};
+    CAP_TRY(leaf_cholinv(ctx, st, (int)n, q.G, n, Rout, q.nr, q.Ri, q.nr, nullptr, 0, &bt));
+  } else {
+    const int64_t mm = q.nb * q.nb;
+    CAP_TRY(sym_pad_batched(ctx, st, n, q.nb, cnt, q.G, q.W));
+    const LeafBatch bt{cnt, {mm, mm, mm, mm}, q.info, batched_cluster_width(q.nb)};
+    CAP_TRY(basecase_cholinv(ctx, st, (int)q.nb, q.W, q.nb, Rout, q.nb, q.Ri, q.nb, q.RiT, q.nb, &bt));
+  }
+  // Q <- Q Rinv: (Q Rinv)^T = Rinv^T Q^T, A = Rinv (upper), B = Q^T
+  GemmBatchOps a;
+  a.batch = cnt; a.A = q.Ri; a.lda = q.nr; a.sa = rr; a.B = QtIn; a.ldb = q.ldt; a.sb = q.ldt * m; a.sc = q.ldt * m; a.sct = sqo;
+  return gemm_tn_batched(ctx, st, n, m, n, 1.0, a, QtOut, q.ldt, QcOut, ldqo, CAPITAL_GEMM_A_UPPER, false);
+}
+
+// C = (L^T)^T U for the upper factors L, U of every matrix (nr x nr each): A = L^T (lower), B = U (upper), upper tiles only
+capital_status_t r_product_batched(QrB& q, const double* L, const double* U, double* Lt, double* C) {
+  const int64_t n = q.n, rr = q.nr * q.nr;
+  CAP_TRY(transpose_batched(q.ctx, q.st, n, n, q.cnt, L, q.nr, rr, Lt, q.nr, rr));
+  GemmBatchOps p;
+  p.batch = q.cnt; p.A = Lt; p.lda = q.nr; p.sa = rr; p.B = U; p.ldb = q.nr; p.sb = rr; p.sc = rr;
+  return gemm_tn_batched(q.ctx, q.st, n, n, n, 1.0, p, C, q.nr, nullptr, 0,
+                         CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER, false);
+}
+}  // namespace
+
+capital_status_t dist_cacqr_factor_batched(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, int num_iter, const double* A, double* Q,
+                                           double* R, int* info) {
+  cudaStream_t st = ctx->stream;
+  QrB q{ctx, st, m, n};
+  q.ldq = round_up(m, 16);
+  q.ldt = round_up(n, 16);
+  q.nr = n <= LEAF_MAX ? round_up(n, 16) : round_up(n, 64);
+  q.nb = round_up(n, 64);
+  // the Gram product reads A in place when TMA can address it (even leading dimension, 16-byte aligned base), as the single path does
+  const bool in_place = !(m & 1) && !((uintptr_t)A & 15);
+  const bool need_q = num_iter > 1 || !in_place;
+  const int64_t rr = q.nr * q.nr, nfac = num_iter == 3 ? 6 : num_iter == 2 ? 5 : 2;  // Ri, R1 (, R2, Rt, R21 (, R3))
+  const int64_t ks = gemm_splitk_chunks(ctx, n, n, m, CAPITAL_GEMM_C_UPPER, nullptr);
+  const int64_t per = (need_q ? q.ldq * n : 0) + q.ldt * m * (num_iter > 1 ? 2 : 1) + n * n + (ks > 1 ? ks * round_up(n, 2) * n : 0) +
+                      nfac * rr + (n > LEAF_MAX ? 2 * q.nb * q.nb : 0);
+  const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>({batch, 65535, QR_BATCHED_CAP / (per * 8)}));
+  auto ws = [&](const char* name, int64_t doubles, double** p) { return ctx->workspace(name, (size_t)(chunk * doubles) * 8, (void**)p); };
+  double *R1, *R2 = nullptr, *R3 = nullptr, *Rt = nullptr, *R21 = nullptr;
+  q.Q = nullptr; q.Qt2 = nullptr; q.W = nullptr; q.RiT = nullptr;
+  if (need_q) CAP_TRY(ws("qrb_Q", q.ldq * n, &q.Q));
+  CAP_TRY(ws("qrb_Qt", q.ldt * m, &q.Qt));
+  if (num_iter > 1) CAP_TRY(ws("qrb_Qt2", q.ldt * m, &q.Qt2));
+  CAP_TRY(ws("qrb_G", n * n, &q.G));
+  CAP_TRY(ws("qrb_Ri", rr, &q.Ri));
+  CAP_TRY(ws("qrb_R1", rr, &R1));
+  if (num_iter > 1) {
+    CAP_TRY(ws("qrb_R2", rr, &R2));
+    CAP_TRY(ws("qrb_Rt", rr, &Rt));
+    CAP_TRY(ws("qrb_R21", rr, &R21));
+  }
+  if (num_iter == 3) CAP_TRY(ws("qrb_R3", rr, &R3));
+  if (n > LEAF_MAX) {
+    CAP_TRY(ws("qrb_W", q.nb * q.nb, &q.W));
+    CAP_TRY(ws("qrb_RiT", q.nb * q.nb, &q.RiT));
+  }
+  CAP_CUDA(cudaMemsetAsync(info, 0, (size_t)batch * sizeof(int), st));
+  const int64_t mn = m * n, sq = q.ldq * n;
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    q.cnt = std::min(chunk, batch - b0);
+    q.info = info + b0;
+    const double* Ab = A + b0 * mn;
+    double* Qb = Q + b0 * mn;
+    const double* Qc = Ab;
+    int64_t ldqc = m, sqc = mn;
+    if (!in_place) {  // the chunk is one m x (cnt n) matrix: one copy to the padded leading dimension
+      CAP_TRY(copy_block(ctx, st, m, q.cnt * n, Ab, m, q.Q, q.ldq));
+      Qc = q.Q; ldqc = q.ldq; sqc = sq;
+    }
+    CAP_TRY(transpose_batched(ctx, st, m, n, q.cnt, Ab, m, mn, q.Qt, q.ldt, q.ldt * m));
+    // the last sweep's transposed store writes Q straight into the output
+    const double* Rfinal = R1;
+    if (num_iter == 3) {
+      CAP_TRY(sweep_batched(q, Qc, ldqc, sqc, q.Qt, q.Qt2, q.Q, q.ldq, sq, R1, scqr3_shift_coef(m, n)));
+      CAP_TRY(sweep_batched(q, q.Q, q.ldq, sq, q.Qt2, q.Qt, q.Q, q.ldq, sq, R2));
+      CAP_TRY(sweep_batched(q, q.Q, q.ldq, sq, q.Qt, nullptr, Qb, m, mn, R3));
+      // R = R3 (R2 R1); R2 R1 goes to a zeroed buffer (C_UPPER leaves its lower part alone, and the second product reads whole
+      // diagonal tiles of its B operand), R3 R21 to R2, free by then
+      CAP_CUDA(cudaMemsetAsync(R21, 0, (size_t)(q.cnt * rr) * 8, st));
+      CAP_TRY(r_product_batched(q, R2, R1, Rt, R21));
+      CAP_TRY(r_product_batched(q, R3, R21, Rt, R2));
+      Rfinal = R2;
+    } else if (num_iter == 2) {
+      CAP_TRY(sweep_batched(q, Qc, ldqc, sqc, q.Qt, q.Qt2, q.Q, q.ldq, sq, R1));
+      CAP_TRY(sweep_batched(q, q.Q, q.ldq, sq, q.Qt2, nullptr, Qb, m, mn, R2));
+      CAP_TRY(r_product_batched(q, R2, R1, Rt, R21));
+      Rfinal = R21;
+    } else {
+      CAP_TRY(sweep_batched(q, Qc, ldqc, sqc, q.Qt, nullptr, Qb, m, mn, R1));
+    }
+    CAP_TRY(triu_out_batched(ctx, st, n, q.cnt, Rfinal, q.nr, rr, R + b0 * n * n));
+  }
+  return CAPITAL_OK;
+}
+
+// X_b = R_b^-1 (Q_b^T B_b), per panel of up to SOLVE_W right-hand sides: the steps of dist_cacqr_apply_qt on one GPU, batched
+capital_status_t dist_cacqr_lstsq_batched(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, const double* Q, const double* R,
+                                          int64_t nrhs, const double* B, double* X) {
+  cudaStream_t st = ctx->stream;
+  // per matrix: tri_apply's partials of Q^T B (64-row owned blocks x 1024-row k chunks x a 64 x 32 tile); the substitution's are smaller
+  const int64_t per = ceil_div(n, 64) * ceil_div(ceil_div(m, 64), 16) * 64 * SOLVE_W * 8;
+  const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>({batch, 65535, QR_BATCHED_CAP / per}));
+  const int64_t mn = m * n, nn = n * n, mk = m * nrhs, nk = n * nrhs;
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+      const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+      double* Xp = X + b0 * nk + p0 * n;
+      //                 U            ldu trans r0 r1 c0 c1 nrhs alpha P                    pinc ldp beta Cin  ldcin C  cinc ldc full batch su  sp  scin sc
+      CAP_TRY(tri_apply(ctx, st, {Q + b0 * mn, m, true, 0, m, 0, n, w, 1.0, B + b0 * mk + p0 * m, 1, m, 0.0, nullptr, 0, Xp, 1, n, true, cnt, mn, mk, 0, nk}));
+      CAP_TRY(tri_solve_batched(ctx, st, R + b0 * nn, n, nn, n, w, Xp, n, nk, cnt));
+    }
+  }
+  return CAPITAL_OK;
+}

@@ -31,6 +31,12 @@ capital_status_t dist_cacqr_apply_q(capital_ctx* ctx, int64_t m, int64_t n, cons
 capital_status_t dist_cacqr_residual(capital_ctx* ctx, const double* A_local, int64_t m, int64_t n, const double* Q_local,
                                      capital_structure_t rstruct, const double* R_local, double* residual, double* orthogonality);
 
+// batched CholeskyQR on this context's GPU (arguments checked by the C entry points)
+capital_status_t dist_cacqr_factor_batched(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, int num_iter, const double* A, double* Q,
+                                           double* R, int* info);
+capital_status_t dist_cacqr_lstsq_batched(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, const double* Q, const double* R,
+                                          int64_t nrhs, const double* B, double* X);
+
 capital_status_t dist_summa_gemm_tn(capital_ctx* ctx, int64_t m, int64_t n, int64_t k, double alpha, const double* A_local,
                                     const double* B_local, double beta, double* C_local);
 

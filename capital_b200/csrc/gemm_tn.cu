@@ -40,6 +40,10 @@ struct GemmParams {
   long long kstride, ldk;
   int no_c;         // skip the store to C (only Ct is wanted)
   GemmXDev x;  // depth exchange fused into the epilogue (XMODE != 0)
+  // batched launches (BATCH): grid z = matrix * ksplit + k chunk; matrix bbase + blockIdx.z / ksplit of the operands' 3D maps writes
+  // C + b sc, Ct + b sct and its split-k partials at kpart + b skp
+  int bbase;
+  long long sc, sct, skp;
 };
 
 struct GemmMaps {
@@ -76,6 +80,12 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+      "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 // D (16 x 8) += A (16 x 16) B (16 x 8), lane (g = lane / 4, q = lane % 4): a[i] = A[g + 8 (i % 2)][q + 4 (i / 2)],
 // b[i] = B[q + 4 i][g], {c0, c1} = D[g][2q, 2q + 1], {c2, c3} = D[g + 8][2q, 2q + 1]
 __device__ __forceinline__ void dmma16816(double& c0, double& c1, double& c2, double& c3, const double2 (&a0)[2], const double2 (&a1)[2],
@@ -93,9 +103,12 @@ constexpr int BK = 16;  // doubles per k tile = one 128-byte swizzle row
 // producer group hands its registers to the consumers (setmaxnreg), which is what lets a 64x32 warp tile
 // (128 accumulator registers) live without spills.
 // XMODE: 0 = plain product; 1 / 2 = depth exchange fused into the epilogue (GemmXDev in common.cuh).
-template <int BM, int BN, int WM, int WN, int STAGES, int MINB, int RC, int RP, int XMODE>
+// BATCH (XMODE 0 only): a batch of independent products of one shape; the operands are 3D tensor maps (k, rows, matrix), so a ragged
+// tile is zero-filled inside its own matrix.  Only the TMA coordinates and the output base offsets differ from the single product.
+template <int BM, int BN, int WM, int WN, int STAGES, int MINB, int RC, int RP, int XMODE, bool BATCH = false>
 __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
     gemm_tn_kernel(const __grid_constant__ GemmMaps maps, const GemmParams p) {
+  static_assert(!BATCH || XMODE == 0, "batched products have no depth exchange");
   constexpr int NWM = BM / WM, NWN = BN / WN, NCW = NWM * NWN;
   constexpr int FM = WM / 8, FN = WN / 8;
   static_assert(FM % 2 == 0, "DMMA.16x8x16 fragments pair the 8-row blocks of a warp tile");
@@ -128,9 +141,12 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
   kb &= ~(BK - 1);
   int nk = ke > kb ? (ke - kb + BK - 1) / BK : 0;
   if (nk == 0 && p.beta == 1.0 && p.ksplit <= 1) return;  // nothing to add (the tile's k range lies outside the operand's triangle); same on every layer
+  // grid z: the k chunk KZ (read where it is used, as blockIdx.z is in the single product) and the matrix bm
+#define KZ (BATCH ? blockIdx.z % (unsigned)p.ksplit : blockIdx.z)
+  const int bm = BATCH ? p.bbase + (int)(blockIdx.z / (unsigned)p.ksplit) : 0;
   if (p.ksplit > 1) {  // this CTA's contiguous chunk of k tiles
     const int per = (nk + p.ksplit - 1) / p.ksplit;
-    const int t0 = min(nk, (int)blockIdx.z * per), t1 = min(nk, t0 + per);
+    const int t0 = min(nk, (int)KZ * per), t1 = min(nk, t0 + per);
     kb += t0 * BK;
     nk = t1 - t0;
     // an empty trailing chunk (ceil(nk / per) < ksplit) runs on with no loads and stores a zero partial: the reduction adds every
@@ -171,8 +187,13 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
           mbar_wait(empty0 + s * 8, ph ^ 1);
           mbar_expect_tx(full0 + s * 8, STAGE_BYTES);
           const int kk = kb + j * BK;
-          tma_load_2d(smem_base + s * STAGE_BYTES, ma, full0 + s * 8, p.rowoffA + kk, m0);
-          tma_load_2d(smem_base + s * STAGE_BYTES + A_BYTES, mb, full0 + s * 8, p.rowoffB + kk, n0);
+          if constexpr (BATCH) {
+            tma_load_3d(smem_base + s * STAGE_BYTES, ma, full0 + s * 8, kk, m0, bm);
+            tma_load_3d(smem_base + s * STAGE_BYTES + A_BYTES, mb, full0 + s * 8, kk, n0, bm);
+          } else {
+            tma_load_2d(smem_base + s * STAGE_BYTES, ma, full0 + s * 8, p.rowoffA + kk, m0);
+            tma_load_2d(smem_base + s * STAGE_BYTES + A_BYTES, mb, full0 + s * 8, p.rowoffB + kk, n0);
+          }
         }
       }
     }
@@ -240,20 +261,20 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
       const int col = n0 + wn * WN + j * 8 + 2 * q + e;
       if (col >= p.N) continue;
       const long long coff = (long long)col * p.ldc;
-      double* cc = p.C + coff;
+      double* cc = (BATCH ? p.C + bm * p.sc : p.C) + coff;
 #pragma unroll
       for (int i = 0; i < FM; i++) {
         const int row = m0 + wm * WM + i * 8 + g;
         if (row >= p.M || (upper_only && row + p.moff > col + p.noff)) continue;
         double v = alpha * acc[i][j][e];
         if (XMODE == 0 && p.ksplit > 1) {
-          if (p.kpart) p.kpart[(long long)blockIdx.z * p.kstride + (long long)col * p.ldk + row] = v;
+          if (p.kpart) (BATCH ? p.kpart + bm * p.skp : p.kpart)[(long long)KZ * p.kstride + (long long)col * p.ldk + row] = v;
           else atomicAdd(cc + row, v);
           continue;
         }
         if (beta != 0.0) v += beta * cc[row];
         if (XMODE != 0 || !p.no_c) cc[row] = v;
-        if (XMODE == 0 && p.Ct) p.Ct[(long long)row * p.ldct + col] = v;
+        if (XMODE == 0 && p.Ct) (BATCH ? p.Ct + bm * p.sct : p.Ct)[(long long)row * p.ldct + col] = v;
         if (XMODE != 0) {  // mode 1: the partner's receive buffer for my partial; mode 2: the partner's replica of C
           for (int oi = 0; oi < nother; oi++) p.x.Cpeer[oi][coff + row] = v;
         }
@@ -261,6 +282,7 @@ __global__ void __launch_bounds__(((BM / WM) * (BN / WN) + 4) * 32, MINB)
     }
   }
   if (XMODE != 0) __threadfence_system();  // the replicas' stores are performed before the kernel retires (the done flag follows on the stream)
+#undef KZ
 }
 
 template <int BM_, int BN_, int WM, int WN, int STAGES, int MINB, int RC, int RP>
@@ -271,6 +293,7 @@ struct GemmCfg {
   static constexpr int smem = STAGES * (BM + BN) * 128 + 2 * STAGES * 8 + 1024;
   template <int XMODE>
   static constexpr auto kernel() { return gemm_tn_kernel<BM, BN, WM, WN, STAGES, MINB, RC, RP, XMODE>; }
+  static constexpr auto kernel_batched() { return gemm_tn_kernel<BM, BN, WM, WN, STAGES, MINB, RC, RP, 0, true>; }
 };
 using CfgBig = GemmCfg<128, 128, 64, 32, 5, 1, 232, 40>;   // 8 consumer warps + producer group, 1 CTA / SM
 using CfgSmall = GemmCfg<64, 64, 32, 32, 6, 1, 0, 0>;       // 4 consumer warps + producer group (a 2-CTA/SM register cap spills the DMMA.16x8x16 fragments)
@@ -353,6 +376,53 @@ capital_status_t launch(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n,
   return CAPITAL_OK;
 }
 
+// 3D map of a batch of k x cols operands (ld, matrix stride s): a box never crosses into the next matrix, whose rows and columns
+// past the operand's edge are zero-filled like those of a single operand
+capital_status_t make_map_3d(capital_ctx* ctx, CUtensorMap* map, const double* base, int64_t rows, int64_t cols, int64_t ld, int64_t s,
+                             int64_t batch, int box_rows_k, int box_cols) {
+  cuuint64_t dims[3] = {(cuuint64_t)rows, (cuuint64_t)cols, (cuuint64_t)batch};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * 8, (cuuint64_t)s * 8};
+  cuuint32_t box[3] = {(cuuint32_t)box_rows_k, (cuuint32_t)box_cols, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = ctx->encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 3, (void*)base, dims, strides, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    ctx->set_error("cuTensorMapEncodeTiled (3D) failed: CUresult " + std::to_string((int)r) + " rows=" + std::to_string(rows) +
+                   " cols=" + std::to_string(cols) + " ld=" + std::to_string(ld) + " stride=" + std::to_string(s) +
+                   " batch=" + std::to_string(batch));
+    return CAPITAL_ERR_CUDA;
+  }
+  return CAPITAL_OK;
+}
+
+// One batched product: grid (tiles, matrices x ksplit), in pieces of at most 65535 / ksplit matrices (grid z)
+template <class Cfg>
+capital_status_t launch_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmBatchOps& b,
+                                double* C, int64_t ldc, int flags, int ksplit, const GemmExtra& ex, long long skp) {
+  constexpr int BM = Cfg::BM, BN = Cfg::BN;
+  GemmParams p{};
+  p.Ct = ex.Ct; p.ldct = ex.ldct; p.no_c = ex.no_c; p.kpart = ex.kpart; p.kstride = ex.kstride; p.ldk = ex.ldk;
+  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = 0.0; p.C = C; p.ldc = ldc; p.ksplit = ksplit;
+  p.ncls = 1;
+  p.sc = b.sc; p.sct = b.sct; p.skp = skp;
+  GemmMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  CAP_TRY(make_map_3d(ctx, &maps.a[0], b.A, k, m, b.lda, b.sa, b.batch, BK, BM));
+  CAP_TRY(make_map_3d(ctx, &maps.b[0], b.B, k, n, b.ldb, b.sb, b.batch, BK, BN));
+  p.gm = (int)ceil_div(m, BM); p.gn = (int)ceil_div(n, BN);
+  const int64_t piece = 65535 / ksplit;
+  for (int64_t b0 = 0; b0 < b.batch; b0 += piece) {
+    const int64_t cnt = std::min(piece, b.batch - b0);
+    p.bbase = (int)b0;
+    dim3 grid((unsigned)p.gm, (unsigned)p.gn, (unsigned)(cnt * ksplit));
+    Cfg::kernel_batched()<<<grid, Cfg::threads, Cfg::smem, st>>>(maps, p);
+    CAP_CUDA(cudaGetLastError());
+    ctx->counters.kernel_launches++;
+  }
+  return CAPITAL_OK;
+}
+
 }  // namespace
 
 // ---- FP64 tensor-pipe ceiling, measured in place ------------------------------------------------------------------
@@ -400,23 +470,44 @@ capital_status_t gemm_tn_init(capital_ctx* ctx) {
   CAP_CUDA(cudaFuncSetAttribute(CfgSmall::kernel<0>(), cudaFuncAttributeMaxDynamicSharedMemorySize, CfgSmall::smem));
   CAP_CUDA(cudaFuncSetAttribute(CfgSmall::kernel<1>(), cudaFuncAttributeMaxDynamicSharedMemorySize, CfgSmall::smem));
   CAP_CUDA(cudaFuncSetAttribute(CfgSmall::kernel<2>(), cudaFuncAttributeMaxDynamicSharedMemorySize, CfgSmall::smem));
+  CAP_CUDA(cudaFuncSetAttribute(CfgBig::kernel_batched(), cudaFuncAttributeMaxDynamicSharedMemorySize, CfgBig::smem));
+  CAP_CUDA(cudaFuncSetAttribute(CfgSmall::kernel_batched(), cudaFuncAttributeMaxDynamicSharedMemorySize, CfgSmall::smem));
   return CAPITAL_OK;
 }
 
 // which tile configuration a product of this output shape runs with
 static inline bool gemm_uses_big(const capital_ctx* ctx, int64_t m, int64_t n) { return ceil_div(m, 128) * ceil_div(n, 128) >= ctx->num_sms; }
 
-// second stage of the deterministic split-k: C = sum over the chunks, in chunk order
+// second stage of the deterministic split-k: C = sum over the chunks, in chunk order.  A batch is the flat outer index: matrix b
+// reads part + b sbp and writes C + b sbc.
 __global__ void splitk_reduce_kernel(long long rows, long long cols, const double* part, long long kstride, long long ldk, int nchunk, double* C,
-                                     long long ldc, int upper_only) {
-  const long long total = rows * cols;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+                                     long long ldc, int upper_only, long long batch, long long sbp, long long sbc) {
+  const long long per = rows * cols, total = per * batch;
+  for (long long gidx = blockIdx.x * (long long)blockDim.x + threadIdx.x; gidx < total; gidx += (long long)gridDim.x * blockDim.x) {
+    const long long b = gidx / per, idx = gidx - b * per;
     const long long c = idx / rows, r = idx - c * rows;
     if (upper_only && r > c) continue;
+    const double* pb = part + b * sbp;
     double s = 0.0;
-    for (int z = 0; z < nchunk; z++) s += part[(long long)z * kstride + c * ldk + r];
-    C[c * ldc + r] = s;
+    for (int z = 0; z < nchunk; z++) s += pb[(long long)z * kstride + c * ldk + r];
+    C[b * sbc + c * ldc + r] = s;
   }
+}
+
+// The split-k chunk count of the Gram product (and its tile): a function of the product's shape and the SM count only, never of a
+// batch, so that a matrix's Gram bits are the same alone and in any batch.
+int64_t gemm_splitk_chunks(const capital_ctx* ctx, int64_t m, int64_t n, int64_t k, int flags, bool* big_out) {
+  const bool big = m >= 128 && n >= 128;
+  const int64_t t = big ? 128 : 64;
+  const int64_t gm = ceil_div(m, t), gn = ceil_div(n, t);
+  int64_t tiles = gm * gn;
+  if ((flags & CAPITAL_GEMM_C_UPPER) && gm == gn) tiles = gm * (gm + 1) / 2;  // tiles below the diagonal return at once
+  int64_t ks = ceil_div((int64_t)ctx->num_sms * (big ? 1 : 2), tiles);
+  const int64_t max_ks = ceil_div(k, 16 * 32);  // at least 32 k-tiles per chunk
+  if (ks > max_ks) ks = max_ks;
+  if (ks < 1) ks = 1;
+  if (big_out) *big_out = big;
+  return ks;
 }
 
 // Split-K variant for short-and-fat products (the tall-skinny Gram matrix, cacqr.hpp:15): C = alpha A^T B with the k range cut
@@ -428,15 +519,8 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
                                 int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc, int flags) {
   if (m <= 0 || n <= 0 || k <= 0) return CAPITAL_OK;
   if (lda < k || ldb < k || ldc < m || (lda & 1) || (ldb & 1)) return CAPITAL_ERR_INVALID;
-  const bool big = m >= 128 && n >= 128;
-  const int64_t t = big ? 128 : 64;
-  const int64_t gm = ceil_div(m, t), gn = ceil_div(n, t);
-  int64_t tiles = gm * gn;
-  if ((flags & CAPITAL_GEMM_C_UPPER) && gm == gn) tiles = gm * (gm + 1) / 2;  // tiles below the diagonal return at once
-  int64_t ks = ceil_div((int64_t)ctx->num_sms * (big ? 1 : 2), tiles);
-  const int64_t max_ks = ceil_div(k, 16 * 32);  // at least 32 k-tiles per chunk
-  if (ks > max_ks) ks = max_ks;
-  if (ks < 1) ks = 1;
+  bool big;
+  const int64_t ks = gemm_splitk_chunks(ctx, m, n, k, flags, &big);
   ctx->counters.kernel_launches += 2;
   ctx->counters.gemm_launches++;
   ctx->counters.gemm_flops += 2.0 * (double)m * (double)n * (double)k * ((flags & CAPITAL_GEMM_C_UPPER) ? 0.5 : 1.0);
@@ -456,8 +540,65 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
   ctx->tl_end(st, tli);
   const long long total = m * n;
   const int gr = (int)std::min<long long>((total + 255) / 256, (long long)ctx->num_sms * 4);
-  splitk_reduce_kernel<<<gr, 256, 0, st>>>(m, n, ex.kpart, ex.kstride, ex.ldk, (int)ks, C, ldc, (flags & CAPITAL_GEMM_C_UPPER) ? 1 : 0);
+  splitk_reduce_kernel<<<gr, 256, 0, st>>>(m, n, ex.kpart, ex.kstride, ex.ldk, (int)ks, C, ldc, (flags & CAPITAL_GEMM_C_UPPER) ? 1 : 0,
+                                           1, 0, 0);
   CAP_CUDA(cudaGetLastError());
+  return CAPITAL_OK;
+}
+
+// A batch of independent products of one shape (batched CholeskyQR, dist.cu).  gram: the split-k Gram product, with the chunk count
+// and tile of gemm_tn_splitk (gemm_splitk_chunks) and its two-stage reduction; otherwise one chunk, alpha A^T B stored into C (ldc
+// >= m, stride sc; C may be nullptr when only Ct is wanted) and, when Ct is set, transposed into Ct (ldct, stride sct) as gemm_tn_t
+// does.  Every matrix gets the bits of the single product of the same shape and flags: the tile may differ from the single
+// product's only where the extra k tiles of a triangular operand add exact zeros.
+capital_status_t gemm_tn_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmBatchOps& b,
+                                 double* C, int64_t ldc, double* Ct, int64_t ldct, int flags, bool gram) {
+  if (m <= 0 || n <= 0 || k <= 0 || b.batch <= 0) return CAPITAL_OK;
+  const bool bad = b.lda < k || b.ldb < k || (b.lda & 1) || (b.ldb & 1) || (b.sa & 1) || (b.sb & 1) || (((uintptr_t)b.A | (uintptr_t)b.B) & 15) ||
+                   (C && ldc < m) || (!C && !Ct) || (Ct && ldct < n) || (gram && (Ct || !C)) || m >= (1LL << 31) || n >= (1LL << 31) ||
+                   k >= (1LL << 31) - 16;
+  if (bad) {
+    ctx->set_error("gemm_tn_batched: invalid operands (16-byte aligned, even leading dimensions and strides, lda, ldb >= k)");
+    return CAPITAL_ERR_INVALID;
+  }
+  ctx->counters.gemm_launches++;
+  double f = 2.0 * (double)m * (double)n * (double)k;
+  const bool atri = flags & (CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_A_LOWER), btri = flags & (CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_B_LOWER);
+  if (atri && btri) f /= 3.0 * ((flags & CAPITAL_GEMM_C_UPPER) && m == n ? 2.0 : 1.0);
+  else if (atri) f = (double)n * (double)m * (double)(m + 1);
+  else if (btri) f = (double)m * (double)n * (double)(n + 1);
+  else if (flags & CAPITAL_GEMM_C_UPPER) f = (double)k * (double)m * (double)(m + 1);
+  ctx->counters.gemm_flops += f * (double)b.batch;
+  GemmExtra ex;
+  ex.Ct = Ct; ex.ldct = ldct; ex.no_c = C ? 0 : 1;
+  if (!gram) {
+    const bool big = m >= 128 && n >= 128 && ceil_div(m, 128) * ceil_div(n, 128) * b.batch >= ctx->num_sms;
+    const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
+    capital_status_t rs;
+    if (big) rs = launch_batched<CfgBig>(ctx, st, m, n, k, alpha, b, C ? C : Ct, C ? ldc : m, flags, 1, ex, 0);
+    else rs = launch_batched<CfgSmall>(ctx, st, m, n, k, alpha, b, C ? C : Ct, C ? ldc : m, flags, 1, ex, 0);
+    ctx->tl_end(st, tli);
+    return rs;
+  }
+  bool big;
+  const int64_t ks = gemm_splitk_chunks(ctx, m, n, k, flags, &big);
+  if (ks == 1) {  // one chunk: the tile is stored straight into C
+    if (big) return launch_batched<CfgBig>(ctx, st, m, n, k, alpha, b, C, ldc, flags, 1, ex, 0);
+    return launch_batched<CfgSmall>(ctx, st, m, n, k, alpha, b, C, ldc, flags, 1, ex, 0);
+  }
+  ex.ldk = round_up(m, 2); ex.kstride = ex.ldk * n;
+  const long long skp = (long long)ks * ex.kstride;
+  CAP_TRY(ctx->workspace("splitk_part_batched", (size_t)(skp * b.batch) * 8, (void**)&ex.kpart));
+  const int tli = ctx->tl_begin(st, big ? 1 : 2, (double)m, (double)n, (double)k);
+  if (big) CAP_TRY((launch_batched<CfgBig>(ctx, st, m, n, k, alpha, b, C, ldc, flags, (int)ks, ex, skp)));
+  else CAP_TRY((launch_batched<CfgSmall>(ctx, st, m, n, k, alpha, b, C, ldc, flags, (int)ks, ex, skp)));
+  ctx->tl_end(st, tli);
+  const long long total = m * n * b.batch;
+  const int gr = (int)std::min<long long>((total + 255) / 256, (long long)ctx->num_sms * 8);
+  splitk_reduce_kernel<<<gr, 256, 0, st>>>(m, n, ex.kpart, ex.kstride, ex.ldk, (int)ks, C, ldc, (flags & CAPITAL_GEMM_C_UPPER) ? 1 : 0,
+                                           b.batch, skp, b.sc);
+  CAP_CUDA(cudaGetLastError());
+  ctx->counters.kernel_launches++;
   return CAPITAL_OK;
 }
 

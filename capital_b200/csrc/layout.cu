@@ -256,6 +256,30 @@ __global__ void __launch_bounds__(SHIFT_T) gram_shift_by_kernel(long long n, dou
   for (long long i = threadIdx.x; i < n; i += SHIFT_T) G[i * ld + i] += s;
 }
 
+__global__ void __launch_bounds__(SHIFT_T) gram_shift_batched_kernel(long long n, double* G, long long ld, long long sg, double coef) {
+  G += (long long)blockIdx.x * sg;
+  const double s = coef * diag_sum_cta(n, G, ld);
+  for (long long i = threadIdx.x; i < n; i += SHIFT_T) G[i * ld + i] += s;
+}
+
+// transpose_kernel on matrix blockIdx.z of a batch
+__global__ void transpose_batched_kernel(int rows, int cols, const double* src, long long lds, long long ss, double* dst, long long ldd,
+                                         long long sd) {
+  __shared__ double tile[TP][TP + 1];
+  src += (long long)blockIdx.z * ss;
+  dst += (long long)blockIdx.z * sd;
+  const int r0 = blockIdx.x * TP, c0 = blockIdx.y * TP;
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int r = r0 + threadIdx.x, c = c0 + j;
+    if (r < rows && c < cols) tile[j][threadIdx.x] = src[(long long)c * lds + r];
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int c = c0 + threadIdx.x, r = r0 + j;
+    if (r < rows && c < cols) dst[(long long)r * ldd + c] = tile[threadIdx.x][j];
+  }
+}
+
 // zero the band |row - col| <= hw of an n x n matrix
 __global__ void zero_band_kernel(long long n, long long hw, double* a, long long ld) {
   const long long w = 2 * hw + 1, total = n * w;
@@ -397,6 +421,23 @@ capital_status_t sub_identity_local(capital_ctx* ctx, cudaStream_t st, int64_t n
 capital_status_t gram_shift(capital_ctx* ctx, cudaStream_t st, int64_t n, double* G, int64_t ld, double coef) {
   if (n <= 0) return CAPITAL_OK;
   gram_shift_kernel<<<1, SHIFT_T, 0, st>>>(n, G, ld, coef);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t gram_shift_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, double* G, int64_t ld, int64_t sg,
+                                    double coef) {
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  if (batch > 65535) return CAPITAL_ERR_INVALID;
+  gram_shift_batched_kernel<<<(unsigned)batch, SHIFT_T, 0, st>>>(n, G, ld, sg, coef);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t transpose_batched(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, int64_t batch, const double* src,
+                                   int64_t lds, int64_t ss, double* dst, int64_t ldd, int64_t sd) {
+  if (rows <= 0 || cols <= 0 || batch <= 0) return CAPITAL_OK;
+  if (batch > 65535 || ceil_div(cols, TP) > 65535) return CAPITAL_ERR_INVALID;
+  dim3 grid((unsigned)ceil_div(rows, TP), (unsigned)ceil_div(cols, TP), (unsigned)batch), block(TP, 8);
+  transpose_batched_kernel<<<grid, block, 0, st>>>((int)rows, (int)cols, src, lds, ss, dst, ldd, sd);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

@@ -10,8 +10,9 @@
 // CTA each, longest blocks first; stage 1 writes one partial per chunk, stage 2 adds the chunks of a block in chunk order and
 // applies alpha, beta.  No atomics anywhere: the same inputs give the same bits (the grid solve relies on it).
 //
-// Batches (cholinv::solve_batched): blockIdx.z of stage 1 and the flat output index of stage 2 pick the matrix; U, P, the partials,
-// Cin and C advance by per-matrix strides.  Batch 1 is the single-matrix call, with the same arithmetic.
+// Batches (cholinv::solve_batched, and with FULL windows cacqr::lstsq_batched): blockIdx.z of stage 1 and the flat output index of
+// stage 2 pick the matrix; U, P, the partials, Cin and C advance by per-matrix strides.  Batch 1 is the single-matrix call, with the
+// same arithmetic.
 //
 // FULL windows (cacqr::apply_QT / apply_Q / lstsq): the same kernel without the j <= i mask and with k over the whole other extent, so
 // a tall rect Q is read once for Q^T P (op T) or Q P (op N).  The substitution Y <- R^-1 Y of lstsq is tri_solve, at the end.
@@ -257,8 +258,8 @@ constexpr int64_t TA_MAX_BLOCKS = 65535;  // owned blocks per launch (grid.y)
 capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x) {
   if (x.nrhs < 1 || x.nrhs > SOLVE_W) { ctx->set_error("tri_apply: 1 <= nrhs <= SOLVE_W"); return CAPITAL_ERR_INVALID; }
   if (x.full && x.ldu == 0) { ctx->set_error("tri_apply: a full window needs rect storage"); return CAPITAL_ERR_INVALID; }
-  if (x.batch < 1 || x.batch > TA_MAX_BLOCKS || (x.batch > 1 && x.full)) {
-    ctx->set_error("tri_apply: 1 <= batch <= 65535, and batches of triangular windows only");
+  if (x.batch < 1 || x.batch > TA_MAX_BLOCKS) {
+    ctx->set_error("tri_apply: 1 <= batch <= 65535");
     return CAPITAL_ERR_INVALID;
   }
   const int64_t o0 = x.trans ? x.c0 : x.r0, o1 = x.trans ? x.c1 : x.r1;
@@ -289,7 +290,8 @@ capital_status_t tri_apply(capital_ctx* ctx, cudaStream_t st, const TriApply& x)
     CAP_TRY(ctx->workspace("solve_part", (size_t)(nob * cmax * TT * w * x.batch) * 8, (void**)&part));
     TriDev a{x.U, x.ldu, x.r0, x.r1, x.c0, x.c1, (int)x.nrhs, x.P, x.pinc, x.ldp, part, nob, cmax, x.su, x.sp, nob * cmax * TT * w};
     const dim3 grid((unsigned)cmax, (unsigned)nob, (unsigned)x.batch);
-    auto launch = x.batch > 1 ? (x.trans ? launch_op<true, false, true> : launch_op<false, false, true>)
+    auto launch = x.batch > 1 ? (x.full ? (x.trans ? launch_op<true, true, true> : launch_op<false, true, true>)
+                                        : (x.trans ? launch_op<true, false, true> : launch_op<false, false, true>))
                   : x.full    ? (x.trans ? launch_op<true, true> : launch_op<false, true>)
                               : (x.trans ? launch_op<true, false> : launch_op<false, false>);
     CAP_TRY(launch(ctx, st, w, a, grid));
@@ -352,11 +354,18 @@ struct SolveDev {
   int nrhs;
   double* Y;
   int64_t ldy;
+  int64_t su, sy;  // per-problem strides (batched kernel)
 };
 
+// BATCH: blockIdx.x is the problem, at strides su (U) and sy (Y) -- a separate instantiation, so the single solve keeps its code
+template <bool BATCH = false>
 __global__ void __launch_bounds__(TS_THREADS) tri_block_solve_kernel(SolveDev a) {
   extern __shared__ double Ts[];       // the triangle, packed
   __shared__ double dinv[TS];          // reciprocals of its diagonal: the chain multiplies
+  if constexpr (BATCH) {
+    a.U += (int64_t)blockIdx.x * a.su;
+    a.Y += (int64_t)blockIdx.x * a.sy;
+  }
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nb = (int)(a.b1 - a.b0);
   const bool packed = a.ldu == 0;
@@ -407,14 +416,35 @@ capital_status_t tri_solve(capital_ctx* ctx, cudaStream_t st, const double* U, i
                            int64_t ldy) {
   if (nrhs < 1 || nrhs > SOLVE_W) { ctx->set_error("tri_solve: 1 <= nrhs <= SOLVE_W"); return CAPITAL_ERR_INVALID; }
   if (n <= 0) return CAPITAL_OK;
-  CAP_CUDA(cudaFuncSetAttribute(tri_block_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TS * (TS + 1) / 2 * 8));
+  CAP_CUDA(cudaFuncSetAttribute(tri_block_solve_kernel<>, cudaFuncAttributeMaxDynamicSharedMemorySize, TS * (TS + 1) / 2 * 8));
   for (int64_t b0 = (n - 1) / TS * TS; b0 >= 0; b0 -= TS) {
     const int64_t b1 = std::min(n, b0 + TS), nb = b1 - b0;
-    tri_block_solve_kernel<<<1, TS_THREADS, (size_t)nb * (nb + 1) / 2 * 8, st>>>(SolveDev{U, ldu, b0, b1, (int)nrhs, Y, ldy});
+    tri_block_solve_kernel<<<1, TS_THREADS, (size_t)nb * (nb + 1) / 2 * 8, st>>>(SolveDev{U, ldu, b0, b1, (int)nrhs, Y, ldy, 0, 0});
     CAP_CUDA(cudaGetLastError());
     ctx->counters.kernel_launches++;
     //                           U  ldu  trans r0  r1  c0  c1  nrhs  alpha P  pinc ldp  beta Cin ldcin C  cinc ldc
     if (b0 > 0) CAP_TRY(tri_apply(ctx, st, {U, ldu, false, 0, b0, b0, b1, nrhs, -1.0, Y, 1, ldy, 1.0, Y, ldy, Y, 1, ldy}));
+  }
+  return CAPITAL_OK;
+}
+
+// The same blocks and updates as tri_solve, one problem per CTA of the block solve and per grid z of the (batched) update
+capital_status_t tri_solve_batched(capital_ctx* ctx, cudaStream_t st, const double* U, int64_t ldu, int64_t su, int64_t n, int64_t nrhs,
+                                   double* Y, int64_t ldy, int64_t sy, int64_t batch) {
+  if (nrhs < 1 || nrhs > SOLVE_W || ldu < n || batch > 65535) {
+    ctx->set_error("tri_solve_batched: 1 <= nrhs <= SOLVE_W, rect U, batch <= 65535");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  CAP_CUDA(cudaFuncSetAttribute(tri_block_solve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TS * (TS + 1) / 2 * 8));
+  for (int64_t b0 = (n - 1) / TS * TS; b0 >= 0; b0 -= TS) {
+    const int64_t b1 = std::min(n, b0 + TS), nb = b1 - b0;
+    tri_block_solve_kernel<true><<<(unsigned)batch, TS_THREADS, (size_t)nb * (nb + 1) / 2 * 8, st>>>(
+        SolveDev{U, ldu, b0, b1, (int)nrhs, Y, ldy, su, sy});
+    CAP_CUDA(cudaGetLastError());
+    ctx->counters.kernel_launches++;
+    //                           U  ldu  trans r0  r1  c0  c1  nrhs  alpha P  pinc ldp  beta Cin ldcin C  cinc ldc  full   batch  su  sp  scin sc
+    if (b0 > 0) CAP_TRY(tri_apply(ctx, st, {U, ldu, false, 0, b0, b0, b1, nrhs, -1.0, Y, 1, ldy, 1.0, Y, ldy, Y, 1, ldy, false, batch, su, sy, sy, sy}));
   }
   return CAPITAL_OK;
 }

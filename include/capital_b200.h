@@ -301,6 +301,25 @@ capital_status_t capital_cacqr_lstsq_f64(capital_ctx* ctx, int64_t m_global, int
                                          capital_structure_t r_structure, const double* R_local, int64_t nrhs,
                                          const double* B_local, int64_t ldb, double* X, int64_t ldx);
 
+/* Batched CholeskyQR on this context's GPU: `batch` independent m x n matrices (1 <= n <= 512, m >= n), each factored A_b = Q_b R_b in
+ * a few launches for the whole batch.  num_iter as in cacqr::factor: 1 = CholeskyQR, 2 = CholeskyQR2, 3 = shifted CholeskyQR3.
+ * A, Q: batch x m x n, column-major, matrix b at offset b m n; R: batch x n x n, written whole (upper triangular, exact zeros below
+ * the diagonal).  info[b] = 0 on success, else the 1-based pivot of the first sweep whose Gram matrix was not positive definite (that
+ * sweep continues with 1 in its place; Q_b and R_b are then unspecified, and the other matrices are unaffected).  Where the single
+ * path's base case is one kernel (n <= 64 or n a multiple of 64), Q_b and R_b have the bits of capital_cacqr_factor_f64 on A_b alone
+ * on one GPU.  Device pointers only; Q must not overlap A.  Enqueued on the context stream without a host synchronisation; never
+ * communicates, so on a grid context each rank factors its own batch.  Intermediates take at most 2 GiB of device memory (more only
+ * when one matrix needs more): larger batches run in chunks.  n > 512: CAPITAL_ERR_UNSUPPORTED; m < n, n < 1, batch < 1, num_iter not
+ * 1, 2 or 3, a NULL argument or a host pointer: CAPITAL_ERR_INVALID. */
+capital_status_t capital_cacqr_factor_batched_f64(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, int num_iter, const double* A,
+                                                  double* Q, double* R, int* info);
+/* X_b = R_b^-1 (Q_b^T B_b) = argmin ||A_b X_b - B_b||_F from the outputs of capital_cacqr_factor_batched_f64.  B: batch x m x nrhs,
+ * X: batch x n x nrhs, column-major, matrix b at offsets b m nrhs and b n nrhs.  Each X_b has the bits of capital_cacqr_lstsq_f64 on
+ * Q_b, R_b (rect) and B_b.  Device pointers only; X must not overlap B.  Enqueued on the context stream; deterministic.  Errors as
+ * the factor (nrhs < 1: CAPITAL_ERR_INVALID). */
+capital_status_t capital_cacqr_lstsq_batched_f64(capital_ctx* ctx, int64_t m, int64_t n, int64_t batch, const double* Q, const double* R,
+                                                 int64_t nrhs, const double* B, double* X);
+
 /* ---- SUMMA ------------------------------------------------------------------------------------ */
 /* matmult::summa::invoke(A, B, C, topo, gemm{Trans, NoTrans, alpha, beta}) -- summa.hpp:6-44 in the T*N form the validators
  * and syrk_internal use (test/cholesky/validate.hpp:35, summa.hpp:143-145):  C = alpha * A^T B + beta * C  with A (k x m),
