@@ -99,7 +99,8 @@ capital_status_t cap_check_info(capital_ctx* ctx) {
     return CAPITAL_ERR_COMM;
   }
   if (info != 0) {
-    ctx->set_error("matrix is not positive definite: non-positive pivot " + std::to_string(info) + " in a base-case block");
+    ctx->set_error("matrix is not positive definite: non-positive pivot " + std::to_string(info) +
+                   " (a column of the matrix on one GPU; on a grid, of the base-case block that failed)");
     return CAPITAL_ERR_NOT_SPD;
   }
   return CAPITAL_OK;

@@ -131,8 +131,9 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
   if (s1 == 0) {
     if (r.hooks && r.hooks->need_cols) CAP_TRY(r.hooks->need_cols(r.hooks->user, r.M, o + n));
     if (pending22) CAP_CUDA(cudaStreamWaitEvent(r.M, pending22, 0));
-    if (n <= LEAF_MAX) CAP_TRY(leaf_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
-    else CAP_TRY(basecase_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit));
+    // info numbers the pivot as a column of the whole matrix: the leaf adds this node's diagonal offset
+    if (n <= LEAF_MAX) CAP_TRY(leaf_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, nullptr, (int)o));
+    else CAP_TRY(basecase_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, nullptr, (int)o));
     return CAPITAL_OK;
   }
   const int64_t s2 = n - s1;

@@ -225,7 +225,8 @@ capital_status_t transpose_batched(capital_ctx* ctx, cudaStream_t st, int64_t ro
 constexpr int LEAF_MAX = 64;
 constexpr int BASECASE_MAX = 512;  // largest block handled by the one-launch cluster kernel (multiple of 64)
 // A batch of independent blocks in one launch: matrix b at W + b s.w, R + b s.r, ... with its own info[b], on clusters of cw CTAs
-// (2, 4 or 8; the cluster kernel only).  Without one (nullptr): a single block, ctx->d_info, width 8.
+// (2, 4 or 8; the cluster kernel only).  Without one (nullptr): a single block, ctx->d_info, width 8.  A failing pivot k of the block
+// is recorded as pivot_base + k + 1: the recursion passes the block's diagonal offset, so that info numbers the column of the whole matrix.
 struct BatchStrides { long long w = 0, r = 0, ri = 0, rit = 0; };
 struct LeafBatch {
   int64_t batch;  // leaf: <= INT32_MAX; cluster kernel: <= 65535 (grid y)
@@ -234,9 +235,10 @@ struct LeafBatch {
   int cw;
 };
 capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, double* W, int64_t ldw, double* R, int64_t ldr,
-                                  double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
+                                  double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr,
+                                  int pivot_base = 0);
 capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const double* W, int64_t ldw, double* R, int64_t ldr,
-                              double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr);
+                              double* Ri, int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt = nullptr, int pivot_base = 0);
 // Cluster width of the batched cluster kernel for nb = 64 T: no phase of the kernel has work for more CTAs than tiles of a block row,
 // and an idle CTA still holds its SM's shared memory.  CAPITAL_BATCHED_CW=8 forces the single-matrix width (measurement).
 static inline int batched_cluster_width(int64_t nb) {

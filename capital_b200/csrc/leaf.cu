@@ -141,7 +141,8 @@ __device__ __forceinline__ void leaf_store(int nb, const double* a, const double
 
 __global__ void __launch_bounds__(256, 1)
     leaf_kernel(int nb, const double* W, long long ldw, double* __restrict__ R, long long ldr, double* __restrict__ Ri,
-                long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, BatchStrides bs) {
+                long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, BatchStrides bs,
+                int pivot_base) {
   extern __shared__ double sm[];
   double* a = sm;
   double* r = sm + LEAF_MAX * LD;
@@ -151,7 +152,7 @@ __global__ void __launch_bounds__(256, 1)
   if (RiT != nullptr) RiT += b * bs.rit;
   leaf_load(nb, W, ldw, a);
   __syncthreads();
-  leaf_factor_invert(nb, a, r, t, info, 0);
+  leaf_factor_invert(nb, a, r, t, info, pivot_base);
   leaf_store(nb, a, r, R, ldr, Ri, ldri, RiT, ldrit);
 }
 
@@ -477,7 +478,7 @@ template <int CW>
 __global__ void __cluster_dims__(CW, 1, 1) __launch_bounds__(256, 1)
     basecase_kernel(int nb, double* __restrict__ W, long long ldw, double* __restrict__ R, long long ldr, double* __restrict__ Ri,
                     long long ldri, double* __restrict__ RiT, long long ldrit, int* __restrict__ info, long long* __restrict__ dbg,
-                    BatchStrides bstr) {
+                    BatchStrides bstr, int pivot_base) {
   {
     const long long b = blockIdx.y;
     W += b * bstr.w; R += b * bstr.r; Ri += b * bstr.ri; RiT += b * bstr.rit; info += b;
@@ -501,7 +502,7 @@ __global__ void __cluster_dims__(CW, 1, 1) __launch_bounds__(256, 1)
     tile_load(sA, W + o + o * ldw, ldw);
     __syncthreads();
     if (dbg && jb == 0 && threadIdx.x == 0) dbg[20] = clock64();
-    leaf64_fast(sA, sB, sT, sU, sm + 4 * TILE_DOUBLES, info, jb * 64, (dbg && jb == 0) ? dbg + 24 : nullptr);
+    leaf64_fast(sA, sB, sT, sU, sm + 4 * TILE_DOUBLES, info, pivot_base + jb * 64, (dbg && jb == 0) ? dbg + 24 : nullptr);
     if (dbg && jb == 0 && threadIdx.x == 0) dbg[21] = clock64();
     tile_store<false>(R + o + o * ldr, ldr, sB);
     tile_store<false>(Ri + o + o * ldri, ldri, sT);
@@ -656,13 +657,13 @@ capital_status_t leaf_init(capital_ctx* ctx) {
 }
 
 capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const double* W, int64_t ldw, double* R, int64_t ldr, double* Ri,
-                              int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt) {
+                              int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt, int pivot_base) {
   if (nb <= 0) return CAPITAL_OK;
   if (nb > LEAF_MAX || (bt && (bt->batch < 1 || bt->batch > INT32_MAX))) return CAPITAL_ERR_INVALID;
   constexpr int smem = LEAF_SMEM;
   const int tli = ctx->tl_begin(st, 4, nb);
   leaf_kernel<<<bt ? (unsigned)bt->batch : 1u, 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, bt ? bt->info : ctx->d_info,
-                                                                bt ? bt->s : BatchStrides{});
+                                                                bt ? bt->s : BatchStrides{}, pivot_base);
   ctx->tl_end(st, tli);
   ctx->counters.kernel_launches++;
   ctx->counters.leaf_launches++;
@@ -672,7 +673,7 @@ capital_status_t leaf_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, const d
 
 // nb must be a multiple of 64, 128 <= nb <= BASECASE_MAX, and RiT non-null.
 capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, double* W, int64_t ldw, double* R, int64_t ldr, double* Ri,
-                                  int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt) {
+                                  int64_t ldri, double* RiT, int64_t ldrit, const LeafBatch* bt, int pivot_base) {
   if (nb % 64 != 0 || nb < 64 || nb > BASECASE_MAX || RiT == nullptr) return CAPITAL_ERR_INVALID;
   const int cw = bt ? bt->cw : 8;
   if (bt && (bt->batch < 1 || bt->batch > 65535)) return CAPITAL_ERR_INVALID;  // grid y
@@ -686,7 +687,7 @@ capital_status_t basecase_cholinv(capital_ctx* ctx, cudaStream_t st, int nb, dou
   }
   const int tli = ctx->tl_begin(st, 3, nb);
   kernel<<<dim3(cw, bt ? (unsigned)bt->batch : 1u), 256, smem, st>>>(nb, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, bt ? bt->info : ctx->d_info,
-                                                                      dbg, bt ? bt->s : BatchStrides{});
+                                                                      dbg, bt ? bt->s : BatchStrides{}, pivot_base);
   ctx->tl_end(st, tli);
   if (dbg) {
     long long h[32];
