@@ -106,7 +106,7 @@ capital_status_t cap_check_info(capital_ctx* ctx) {
   return CAPITAL_OK;
 }
 
-// ---- host-pointer streaming of cholinv::factor (single GPU) ----------------------------------------------------
+// ---- column streaming of cholinv::factor (single GPU): A in, R and Rinv out --------------------------------------
 namespace {
 struct HostIO {
   capital_ctx* ctx = nullptr;
@@ -117,6 +117,8 @@ struct HostIO {
   int64_t waited = 0;
   int64_t cols_out = 0, rinv_cols_out = 0;
   bool rinv_streams = false;  // Rinv columns right of the top split are final as soon as R's are (complete_inv == 0)
+  int64_t rinv_top = 0;       // complete_inv == 0, packed: rows [0, rinv_top) of Rinv's columns from rinv_top on are the skipped block,
+                              // zeroed in the output once at the start; the packs leave them alone
   cudaEvent_t e_out = nullptr;
 };
 capital_status_t io_event(capital_ctx* ctx, cudaEvent_t* e) {
@@ -128,17 +130,25 @@ capital_status_t io_event(capital_ctx* ctx, cudaEvent_t* e) {
   *e = ctx->io_pool[ctx->io_used++];
   return CAPITAL_OK;
 }
-capital_status_t hostio_need_cols(void* user, cudaStream_t st, int64_t col_end) {
-  HostIO* io = (HostIO*)user;
+// make st wait for the first chunk that covers columns [0, col_end); returns that chunk's end
+capital_status_t hostio_wait_chunk(HostIO* io, cudaStream_t st, int64_t col_end, int64_t* waited) {
   capital_ctx* ctx = io->ctx;
-  if (col_end <= io->waited) return CAPITAL_OK;
   for (auto& ch : io->chunks)
     if (ch.first >= col_end) {
       CAP_CUDA(cudaStreamWaitEvent(st, ch.second, 0));
-      io->waited = ch.first;
+      *waited = ch.first;
       return CAPITAL_OK;
     }
   return CAPITAL_OK;
+}
+capital_status_t hostio_need_cols(void* user, cudaStream_t st, int64_t col_end) {
+  HostIO* io = (HostIO*)user;
+  if (col_end <= io->waited) return CAPITAL_OK;
+  return hostio_wait_chunk(io, st, col_end, &io->waited);
+}
+capital_status_t hostio_wait_cols(void* user, cudaStream_t st, int64_t col_end) {
+  int64_t waited = 0;
+  return hostio_wait_chunk((HostIO*)user, st, col_end, &waited);
 }
 // columns [cols_out, col_end) of R are final (and of Rinv too when the top-level inverse block is skipped, complete_inv == 0:
 // then Rinv's columns right of the top split only hold the right child's own inverse): pack them -- a contiguous range of
@@ -163,7 +173,7 @@ capital_status_t hostio_left_done(void* user, cudaStream_t st, int64_t col_end, 
     CAP_CUDA(cudaStreamWaitEvent(ps, e, 0));
   }
   CAP_TRY(pack_upper(ctx, ps, io->L, io->Rm, io->ld, io->dR, 0, c0, col_end));
-  if (rinv_too) CAP_TRY(pack_upper(ctx, ps, io->L, io->Ri, io->ld, io->dRinv, 0, c0, col_end));
+  if (rinv_too) CAP_TRY(pack_upper(ctx, ps, io->L, io->Ri, io->ld, io->dRinv, 0, c0, col_end, io->rinv_top));
   io->cols_out = col_end;
   if (rinv_too) io->rinv_cols_out = col_end;
   if (!io->hR && !io->hRinv) {  // device outputs: nothing to copy out
@@ -183,6 +193,28 @@ capital_status_t hostio_left_done(void* user, cudaStream_t st, int64_t col_end, 
   return CAPITAL_OK;
 }
 int64_t hostio_cols_waited(void* user) { return ((HostIO*)user)->waited; }
+// all of R is final (the last base case has been issued on st): its columns not packed yet are packed, and copied out, on the copy-out
+// stream while the chain still computes the inverse blocks of the right spine
+capital_status_t hostio_r_final(void* user, cudaStream_t st) {
+  HostIO* io = (HostIO*)user;
+  capital_ctx* ctx = io->ctx;
+  const int64_t c0 = io->cols_out;
+  if (c0 >= io->L || ctx->no_overlap) return CAPITAL_OK;
+  cudaEvent_t e;
+  CAP_TRY(io_event(ctx, &e));
+  CAP_CUDA(cudaEventRecord(e, st));
+  CAP_CUDA(cudaStreamWaitEvent(ctx->copy_out, e, 0));
+  CAP_TRY(pack_upper(ctx, ctx->copy_out, io->L, io->Rm, io->ld, io->dR, 0, c0, io->L));
+  io->cols_out = io->L;
+  if (io->hR) {
+    const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = (size_t)io->L * (io->L + 1) / 2 - off;
+    CAP_CUDA(cudaMemcpyAsync(io->hR + off, io->dR + off, cnt * 8, cudaMemcpyDeviceToHost, ctx->copy_out));
+    ctx->counters.d2h_bytes += (int64_t)cnt * 8;
+  }
+  CAP_TRY(io_event(ctx, &io->e_out));
+  CAP_CUDA(cudaEventRecord(io->e_out, ctx->copy_out));
+  return CAPITAL_OK;
+}
 // pack columns [done, col_end) of R (or Rinv) on the chain and queue their D2H on the copy-out stream (host outputs only)
 capital_status_t hostio_emit(HostIO* io, cudaStream_t st, bool r_part, int64_t col_end) {
   capital_ctx* ctx = io->ctx;
@@ -193,7 +225,7 @@ capital_status_t hostio_emit(HostIO* io, cudaStream_t st, bool r_part, int64_t c
   double* dev = r_part ? io->dR : io->dRinv;
   double* host = r_part ? io->hR : io->hRinv;
   const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = (size_t)col_end * (col_end + 1) / 2 - off;
-  CAP_TRY(pack_upper(ctx, st, io->L, src, io->ld, dev, 0, c0, col_end));
+  CAP_TRY(pack_upper(ctx, st, io->L, src, io->ld, dev, 0, c0, col_end, r_part ? 0 : io->rinv_top));
   done = col_end;
   if (!host) return CAPITAL_OK;
   cudaEvent_t e;
@@ -536,58 +568,75 @@ capital_status_t capital_cholinv_factor_f64(capital_ctx* ctx, const double* A_lo
   CAP_TRY(cap_stage_out_begin(ctx, Rinv_local, out_count, "Rinv_out", &dRinv));
   CAP_CUDA(cudaMemsetAsync(ctx->d_info, 0, sizeof(int), st));
   const int64_t bc = capital_cholinv_bc_dimension(L, g.c, g.d, args->bc_mult_dim);
-  if (ostruct == CAPITAL_RECT) {
-    CAP_CUDA(cudaMemsetAsync(Ri, 0, (size_t)ld * L * 8, st));  // rect outputs expose everything
-  } else {
-    CAP_TRY(zero_band(ctx, st, L, Ri, ld));
-    // the skipped top-level block of Rinv (cholinv.hpp:147) must read as zeros in the packed output -- it only exists when the top
-    // node splits (same predicate as cholinv_local: a top-level base case returns the full inverse)
-    if (args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split)) {
-      const int64_t s1 = L >> args->split;
-      if (s1 > 0 && s1 < L) CAP_TRY(zero_block(ctx, st, s1, L - s1, Ri + s1 * ld, ld));
-    }
-  }
+  // the top-level block of Rinv that complete_inv = 0 skips (cholinv.hpp:147) -- it only exists when the top node splits (same
+  // predicate as cholinv_local: a top-level base case returns the full inverse).  Nothing in the factorization reads it: the packed
+  // output gets its zeros without reading the workspace (zero_packed_top below), the rect output exposes the whole buffer and clears it.
+  const bool skipped = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
+  if (ostruct == CAPITAL_RECT) CAP_CUDA(cudaMemsetAsync(Ri, 0, (size_t)ld * L * 8, st));
+  else CAP_TRY(zero_band(ctx, st, L, Ri, ld));
   CAP_TRY(zero_band(ctx, st, L, RiT, ld));
   if (ostruct == CAPITAL_RECT) CAP_CUDA(cudaMemsetAsync(Rm, 0, (size_t)ld * L * 8, st));
 
-  // Host-pointer callers: A streams in by column chunks on a copy stream while the recursion already works on the leading
-  // columns (it consumes W left to right); the finished left half of R / Rinv streams out while the right half computes.
+  // A streams into W by column chunks on the copy-in stream while the recursion already works on the leading columns (it consumes
+  // W left to right): the chain waits for each chunk where it first reads its columns, so the first base case starts after the
+  // first, narrow chunk instead of after the whole copy.  Device input is copied too (the caller's A is not destroyed).
+  // The finished left half of R / Rinv is packed (and, for host outputs, copied out) while the right half computes.
   HostIO io;
   io.ctx = ctx; io.L = L; io.ld = ld; io.Rm = Rm; io.Ri = Ri; io.dR = dR; io.dRinv = dRinv;
   io.hR = (dR != R_local) ? R_local : nullptr; io.hRinv = (dRinv != Rinv_local) ? Rinv_local : nullptr;
   io.packed = ostruct == CAPITAL_UPPERTRI_PACKED;
-  io.rinv_streams = args->complete_inv == 0 && cholinv_node_splits(L, bc, (int)args->split);
-  CholinvHooks hooks{&io, nullptr, nullptr};
-  if (!cap_is_device_ptr(A_local)) {
+  io.rinv_streams = skipped;
+  io.rinv_top = skipped && io.packed ? L >> args->split : 0;
+  CholinvHooks hooks{&io, hostio_need_cols, nullptr};
+  hooks.wait_cols = hostio_wait_cols;
+  const bool host_in = !cap_is_device_ptr(A_local);
+  cudaEvent_t e_zero = nullptr;
+  {
     cudaEvent_t e0;
     CAP_TRY(io_event(ctx, &e0));
-    CAP_CUDA(cudaEventRecord(e0, st));  // W must be free (previous users on st) before the copies land
+    CAP_CUDA(cudaEventRecord(e0, st));  // W and the outputs must be free (previous users on st) before the copies land
     CAP_CUDA(cudaStreamWaitEvent(ctx->copy_in, e0, 0));
+    if (io.rinv_top) {
+      // the zeros of the skipped Rinv block depend on nothing: they are written beside the first base cases, off the chain and out
+      // of the final pack (the copy-out stream's packs and copies of finished columns queue behind them)
+      CAP_CUDA(cudaStreamWaitEvent(ctx->copy_out, e0, 0));
+      CAP_TRY(zero_packed_top(ctx, ctx->copy_out, L, dRinv, io.rinv_top));
+      CAP_TRY(io_event(ctx, &e_zero));
+      CAP_CUDA(cudaEventRecord(e_zero, ctx->copy_out));
+    }
     const int64_t chunk = round_up(ceil_div(L, 16), 64);
-    for (int64_t c0 = 0; c0 < L; c0 += chunk) {
-      const int64_t nc = (c0 + chunk <= L) ? chunk : L - c0;
-      // only the upper triangle of A is read (serialize<uppertri>(A -> R), cholinv.hpp:13): rows [0, c0 + nc) of this chunk
+    for (int64_t c0 = 0; c0 < L;) {
+      // the first base case reads only its own columns: a narrow first chunk lets it start almost at once
+      const int64_t nc = std::min(c0 == 0 ? std::min<int64_t>(chunk, 512) : chunk, L - c0);
+      // only the upper triangle of A is read (serialize<uppertri>(A -> R), cholinv.hpp:13): rows [0, c0 + nc) of this chunk.  The
+      // strictly lower blocks of W are the scratch for T^T, written before they are read.
       const int64_t rows = c0 + nc;
+      const int tli = ctx->tl_begin(ctx->copy_in, 8, 2, (double)rows, (double)nc);
       CAP_CUDA(cudaMemcpy2DAsync(W + c0 * ld, (size_t)ld * 8, A_local + c0 * L, (size_t)L * 8, (size_t)rows * 8, (size_t)nc,
-                                 cudaMemcpyHostToDevice, ctx->copy_in));
-      ctx->counters.h2d_bytes += rows * nc * 8;
+                                 host_in ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, ctx->copy_in));
+      ctx->tl_end(ctx->copy_in, tli);
+      if (host_in) ctx->counters.h2d_bytes += rows * nc * 8;
       cudaEvent_t e;
       CAP_TRY(io_event(ctx, &e));
       CAP_CUDA(cudaEventRecord(e, ctx->copy_in));
       io.chunks.push_back({c0 + nc, e});
+      c0 += nc;
     }
-    hooks.need_cols = hostio_need_cols;
-  } else {
-    CAP_TRY(copy_block(ctx, st, L, L, A_local, L, W, ld));  // serialize(A -> R), cholinv.hpp:13
   }
-  if (io.packed && L >= 2048) hooks.left_done = hostio_left_done;  // finished column ranges are packed (and copied out) early
-  if (hooks.need_cols) hooks.cols_waited = hostio_cols_waited;
+  if (io.packed && L >= 2048) {  // finished column ranges are packed (and copied out) early
+    hooks.left_done = hostio_left_done;
+    hooks.r_final = hostio_r_final;
+  }
+  // Host input arrives at PCIe speed: R12 products are issued by column chunks that follow it (and there are no bands).  Device input
+  // has arrived long before any R12: the products are issued whole, with their leading bands.
+  if (host_in) hooks.cols_waited = hostio_cols_waited;
   if (hooks.left_done && (io.hR || io.hRinv)) {  // host outputs: the tail of R and the top-level inverse block stream out too
     hooks.right_done = hostio_right_done;
     if (io.hRinv) hooks.inv_cols = hostio_inv_cols;
   }
   CAP_TRY(cholinv_local(ctx, st, L, W, ld, Rm, ld, Ri, ld, RiT, ld, args->complete_inv != 0, bc, (int)args->split, &hooks));
   if (ostruct == CAPITAL_UPPERTRI_PACKED) {
+    if (e_zero) CAP_CUDA(cudaStreamWaitEvent(st, e_zero, 0));
     {  // columns [0, c0) are already packed (and on their way to the host)
       const int64_t c0 = io.cols_out;
       const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = out_count - off;
@@ -597,7 +646,7 @@ capital_status_t capital_cholinv_factor_f64(capital_ctx* ctx, const double* A_lo
     {
       const int64_t c0 = io.rinv_cols_out;
       const size_t off = (size_t)c0 * (c0 + 1) / 2, cnt = out_count - off;
-      CAP_TRY(pack_upper(ctx, st, L, Ri, ld, dRinv, 0, c0, L));
+      CAP_TRY(pack_upper(ctx, st, L, Ri, ld, dRinv, 0, c0, L, io.rinv_top));
       if (io.hRinv && cnt) { CAP_CUDA(cudaMemcpyAsync(io.hRinv + off, dRinv + off, cnt * 8, cudaMemcpyDeviceToHost, st)); ctx->counters.d2h_bytes += (int64_t)cnt * 8; }
     }
     if (io.e_out) CAP_CUDA(cudaStreamWaitEvent(st, io.e_out, 0));  // the early D2H of the left half

@@ -54,7 +54,12 @@ struct Rec {
   int64_t band_min;   // nodes whose left part is smaller than this issue their products whole
   int64_t total;      // size of the top-level block
   bool base_aligned;  // all four buffers 16-byte aligned with even leading dimensions (cluster kernel uses 16-byte accesses)
+  // A node's T^T reads the RiT of its left child only, so the RiT21 blocks of the right spine (o + n == total) are read by nobody
+  // when the top node skips its Rinv12 (complete_inv = 0): they are not written then.
+  bool spine_rit;
 };
+
+bool writes_rit21(const Rec& r, int64_t o, int64_t n) { return r.spine_rit || o + n != r.total; }
 
 // Levels above the base case (n > bc) split by the reference's rule s1 = n >> split (cholinv.hpp:92,107); it fixes
 // which Rinv block stays zero when complete_inv == 0.  Below it -- the reference's potrf/trtri base case
@@ -102,14 +107,15 @@ capital_status_t issue_band(Rec& r, Band& b, int64_t split) {
   const int64_t ldw = r.ldw, ldr = r.ldr, ldri = r.ldri, ldrit = r.ldrit;
   double* Ri = r.Ri + o * ldri + o;
   if (b.r12) {
-    // R12[0:edge, :] = Rinv11[0:edge, 0:edge]^T A12[0:edge, :]
+    // R12[0:edge, :] = Rinv11[0:edge, 0:edge]^T A12[0:edge, :], once A12 has arrived
+    if (r.hooks && r.hooks->wait_cols) CAP_TRY(r.hooks->wait_cols(r.hooks->user, b.st, o + s1 + s2));
     CAP_TRY(gemm_tn(ctx, b.st, edge, s2, edge, 1.0, Ri, ldri, r.W + (o + s1) * ldw + o, ldw, 0.0, r.R + (o + s1) * ldr + o, ldr,
                     CAPITAL_GEMM_A_UPPER));
   } else {
     // Rinv12[:, 0:edge] = -(T^T)^T Rinv22[0:edge, 0:edge]
     double* Ri12 = Ri + s1 * ldri;
     CAP_TRY(gemm_tn(ctx, b.st, s1, edge, edge, -1.0, r.W + o * ldw + o + s1, ldw, Ri12 + s1, ldri, 0.0, Ri12, ldri, CAPITAL_GEMM_B_UPPER));
-    CAP_TRY(transpose_block(ctx, b.st, s1, edge, Ri12, ldri, r.RiT + o * ldrit + o + s1, ldrit, 1.0));
+    if (writes_rit21(r, o, s1 + s2)) CAP_TRY(transpose_block(ctx, b.st, s1, edge, Ri12, ldri, r.RiT + o * ldrit + o + s1, ldrit, 1.0));
   }
   CAP_TRY(new_event(ctx, &b.done));
   CAP_CUDA(cudaEventRecord(b.done, b.st));
@@ -134,6 +140,7 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
     // info numbers the pivot as a column of the whole matrix: the leaf adds this node's diagonal offset
     if (n <= LEAF_MAX) CAP_TRY(leaf_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, nullptr, (int)o));
     else CAP_TRY(basecase_cholinv(ctx, r.M, (int)n, W, ldw, R, ldr, Ri, ldri, RiT, ldrit, nullptr, (int)o));
+    if (o + n == r.total && r.hooks && r.hooks->r_final) CAP_TRY(r.hooks->r_final(r.hooks->user, r.M));
     return CAPITAL_OK;
   }
   const int64_t s2 = n - s1;
@@ -249,7 +256,7 @@ capital_status_t rec(Rec& r, int64_t o, int64_t n, bool complete, cudaEvent_t pe
       CAP_TRY(gemm_tn_off(ctx, r.M, s1, s2 - c, s2, -1.0, W21, ldw, Ri22 + c * ldri, ldri, 0.0, Ri12 + c * ldri, ldri, CAPITAL_GEMM_B_UPPER,
                           (int)c));
     }
-    CAP_TRY(transpose_block(ctx, r.M, s1, s2 - bi.edge, Ri12 + bi.edge * ldri, ldri, RiT21 + bi.edge, ldrit, 1.0));
+    if (writes_rit21(r, o, n)) CAP_TRY(transpose_block(ctx, r.M, s1, s2 - bi.edge, Ri12 + bi.edge * ldri, ldri, RiT21 + bi.edge, ldrit, 1.0));
     if (bi.done) CAP_CUDA(cudaStreamWaitEvent(r.M, bi.done, 0));
   }
   return CAPITAL_OK;
@@ -264,8 +271,8 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
   cudaStream_t M = (ctx->hi && allow_side) ? ctx->hi : st;
   cudaStream_t S = (allow_side && ctx->hi && ctx->side && n >= 1024 && !ctx->no_overlap) ? ctx->side : nullptr;
   cudaStream_t D = S ? ctx->side_deep[0] : nullptr, T = S ? ctx->side_deep[1] : nullptr;
-  // no bands while A is still arriving from the host: there the R12 products follow the arrival of their columns instead
-  const bool bands = S && !(hooks && hooks->need_cols);
+  // no bands while A arrives from the host: there the R12 products follow the arrival of their columns instead
+  const bool bands = S && !(hooks && hooks->cols_waited);
   ctx->dep_used = 0;
   cudaEvent_t e_in = nullptr, e_out = nullptr, e_s = nullptr;
   if (M != st) {
@@ -279,6 +286,7 @@ capital_status_t cholinv_local(capital_ctx* ctx, cudaStream_t st, int64_t n, dou
   // a top-level node the reference treats as its base case (n <= bc, cholinv.hpp:93-104) gets the FULL inverse whatever complete_inv
   // says; the skip of cholinv.hpp:147 only exists where the top node really splits at n >> split
   if (!cholinv_node_splits(n, bc, split)) complete_top = true;
+  r.spine_rit = complete_top;
   CAP_TRY(rec(r, 0, n, complete_top, nullptr, nullptr, 0, nullptr));
   if (M != st) {
     if (S) {  // join the deferred streams (all their work has been consumed through events, this is just the fence)

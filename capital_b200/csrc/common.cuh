@@ -178,8 +178,12 @@ capital_status_t copy_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, int
                             double* dst, int64_t ldd);
 capital_status_t zero_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, double* dst, int64_t ldd);
 capital_status_t zero_band(capital_ctx* ctx, cudaStream_t st, int64_t n, double* a, int64_t ld);
+// columns [col_begin, col_end) of the upper triangle of src into the packed triangle; with skip_top > 0, rows [0, skip_top) of the
+// columns from skip_top on are neither read nor written (the top-level block of Rinv that complete_inv = 0 skips: zero_packed_top)
 capital_status_t pack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* packed,
-                            int zero_diag, int64_t col_begin = 0, int64_t col_end = -1);
+                            int zero_diag, int64_t col_begin = 0, int64_t col_end = -1, int64_t skip_top = 0);
+// zeros into rows [0, top) of the packed columns [top, n)
+capital_status_t zero_packed_top(capital_ctx* ctx, cudaStream_t st, int64_t n, double* packed, int64_t top);
 capital_status_t unpack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* packed, double* dst, int64_t ldd);
 capital_status_t triu_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst,
                            int64_t ldd, int zero_diag);
@@ -250,20 +254,24 @@ static inline int batched_cluster_width(int64_t nb) {
 
 // ---- cholinv.cu -------------------------------------------------------------------------------
 // local (single-GPU) recursive CholInv on dense n x n blocks; W is destroyed (Schur complements).
-// Optional callbacks of the top-level call (host-pointer path): `need_cols` makes `st` wait until columns [0, col_end)
-// of W have arrived from the host; `left_done` fires after each left child on the right spine (depth <= 3), when columns
+// Optional callbacks of the top-level call (cholinv::factor on one GPU): `need_cols` makes the chain's stream `st` wait until
+// columns [0, col_end) of W have arrived; `left_done` fires after each left child on the right spine (depth <= 3), when columns
 // [0, col_end) of R are final, and those of Rinv too at depth 0.
 struct CholinvHooks {
   void* user;
   capital_status_t (*need_cols)(void* user, cudaStream_t st, int64_t col_end);
   capital_status_t (*left_done)(void* user, cudaStream_t st, int64_t col_end, int depth);
-  // optional (host-pointer callers).  `cols_waited`: how many leading columns the chain already waited for -- while it is short of a
+  // optional.  `wait_cols`: as need_cols, for a stream other than the chain (the leading band of an R12 product).
+  // `cols_waited` (host input): how many leading columns the chain already waited for -- while it is short of a
   // node's extent, the node's R12 product is issued in column chunks, each behind the arrival of its own columns only.
   // `right_done`: the top-level right child has returned, all of R is final.  `inv_cols`: the top-level inverse block is issued in
   // column chunks; columns [0, col_end) of Rinv are final.
   int64_t (*cols_waited)(void* user);
   capital_status_t (*right_done)(void* user, cudaStream_t st);
   capital_status_t (*inv_cols)(void* user, cudaStream_t st, int64_t col_end);
+  capital_status_t (*wait_cols)(void* user, cudaStream_t st, int64_t col_end);
+  // `r_final`: the last base case (bottom of the right spine) has been issued on `st`, all of R is final after it.
+  capital_status_t (*r_final)(void* user, cudaStream_t st);
 };
 // allow_side = false keeps everything on `st` (the distributed base case runs on the critical chain and must not queue behind
 // the deferred stream's GEMMs).

@@ -43,13 +43,21 @@ __global__ void zero_kernel(long long rows, long long cols, double* dst, long lo
   }
 }
 
-// one block per column chunk: column i of the packed triangle is contiguous (i+1 entries at i(i+1)/2)
+// one block per column chunk: column i of the packed triangle is contiguous (i+1 entries at i(i+1)/2); rows [0, skip_top) of the
+// columns from skip_top on are neither read nor written
 __global__ void pack_upper_kernel(long long c0, long long n, const double* src, long long lds, double* packed,
-                                  int zero_diag) {
+                                  int zero_diag, long long skip_top) {
   for (long long i = c0 + blockIdx.x; i < n; i += gridDim.x) {
     const double* s = src + i * lds;
     double* d = packed + i * (i + 1) / 2;
-    for (long long j = threadIdx.x; j <= i; j += blockDim.x) d[j] = (zero_diag && j == i) ? 0.0 : s[j];
+    for (long long j = (i >= skip_top ? skip_top : 0) + threadIdx.x; j <= i; j += blockDim.x) d[j] = (zero_diag && j == i) ? 0.0 : s[j];
+  }
+}
+// rows [0, top) of the packed columns [top, n)
+__global__ void zero_packed_top_kernel(long long top, long long n, double* packed) {
+  for (long long i = top + blockIdx.x; i < n; i += gridDim.x) {
+    double* d = packed + i * (i + 1) / 2;
+    for (long long j = threadIdx.x; j < top; j += blockDim.x) d[j] = 0.0;
   }
 }
 __global__ void unpack_upper_kernel(long long n, const double* packed, double* dst, long long ldd) {
@@ -280,12 +288,11 @@ __global__ void transpose_batched_kernel(int rows, int cols, const double* src, 
   }
 }
 
-// zero the band |row - col| <= hw of an n x n matrix
+// zero the band |row - col| <= hw of an n x n matrix: one block per column, contiguous rows
 __global__ void zero_band_kernel(long long n, long long hw, double* a, long long ld) {
-  const long long w = 2 * hw + 1, total = n * w;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
-    const long long c = idx / w, r = c - hw + (idx - c * w);
-    if (r >= 0 && r < n) a[c * ld + r] = 0.0;
+  for (long long c = blockIdx.x; c < n; c += gridDim.x) {
+    const long long r0 = c - hw > 0 ? c - hw : 0, r1 = c + hw < n - 1 ? c + hw : n - 1;
+    for (long long r = r0 + threadIdx.x; r <= r1; r += blockDim.x) a[c * ld + r] = 0.0;
   }
 }
 
@@ -341,12 +348,23 @@ capital_status_t zero_block(capital_ctx* ctx, cudaStream_t st, int64_t rows, int
   return CAPITAL_OK;
 }
 capital_status_t pack_upper(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* packed, int zero_diag,
-                            int64_t col_begin, int64_t col_end) {
+                            int64_t col_begin, int64_t col_end, int64_t skip_top) {
   if (col_end < 0) col_end = n;
+  if (skip_top <= 0) skip_top = n;
   const int64_t cols = col_end - col_begin;
   if (cols <= 0) return CAPITAL_OK;
   const int tli = ctx->tl_begin(st, 8, 3, (double)col_begin, (double)col_end);
-  pack_upper_kernel<<<(int)(cols < ctx->num_sms * 8 ? cols : ctx->num_sms * 8), 256, 0, st>>>(col_begin, col_end, src, lds, packed, zero_diag);
+  pack_upper_kernel<<<(int)(cols < ctx->num_sms * 8 ? cols : ctx->num_sms * 8), 256, 0, st>>>(col_begin, col_end, src, lds, packed, zero_diag,
+                                                                                              skip_top);
+  ctx->tl_end(st, tli);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t zero_packed_top(capital_ctx* ctx, cudaStream_t st, int64_t n, double* packed, int64_t top) {
+  if (top <= 0 || top >= n) return CAPITAL_OK;
+  const int64_t cols = n - top;
+  const int tli = ctx->tl_begin(st, 8, 4, (double)top, (double)n);
+  zero_packed_top_kernel<<<(int)(cols < ctx->num_sms * 8 ? cols : ctx->num_sms * 8), 256, 0, st>>>(top, n, packed);
   ctx->tl_end(st, tli);
   LAUNCH_CHECK();
   return CAPITAL_OK;
@@ -464,7 +482,9 @@ capital_status_t zero_band(capital_ctx* ctx, cudaStream_t st, int64_t n, double*
     CAP_CUDA(cudaMemsetAsync(a, 0, (size_t)ld * n * 8, st));
     return CAPITAL_OK;
   }
-  zero_band_kernel<<<grid_for(ctx, n * (2 * hw + 1), 256), 256, 0, st>>>(n, hw, a, ld);
+  const int tli = ctx->tl_begin(st, 8, 5, (double)n, (double)hw);
+  zero_band_kernel<<<(int)(n < ctx->num_sms * 8 ? n : ctx->num_sms * 8), 256, 0, st>>>(n, hw, a, ld);
+  ctx->tl_end(st, tli);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }
