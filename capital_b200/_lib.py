@@ -18,6 +18,8 @@ EXPORTS = [  # every symbol include/capital_b200.h declares
     "capital_distribute_random_f64", "capital_cholinv_factor_f64", "capital_cholinv_residual_f64", "capital_cholinv_solve_f64",
     "capital_cholinv_inverse_f64", "capital_cholinv_inverse_residual_f64", "capital_cholinv_sygst_f64", "capital_cholinv_apply_rinv_f64",
     "capital_cholinv_sygst_ab_f64", "capital_cholinv_apply_r_f64", "capital_cholinv_factor_batched_f64", "capital_cholinv_solve_batched_f64",
+    "capital_cholinv_inverse_batched_f64", "capital_cholinv_sygst_batched_f64", "capital_cholinv_sygst_ab_batched_f64",
+    "capital_cholinv_apply_rinv_batched_f64", "capital_cholinv_apply_r_batched_f64",
     "capital_cacqr_factor_f64", "capital_cacqr_residual_f64", "capital_cacqr_apply_qt_f64", "capital_cacqr_apply_q_f64",
     "capital_cacqr_lstsq_f64", "capital_cacqr_factor_batched_f64", "capital_cacqr_lstsq_batched_f64", "capital_summa_gemm_tn_f64", "capital_blas_gemm_tn_f64",
     "capital_lapack_potrf_trtri_f64",
@@ -104,6 +106,11 @@ def lib() -> C.CDLL:
     L.capital_cholinv_apply_r_f64.argtypes = [vp, i64, C.POINTER(CholinvArgs), ci, vp, ci, i64, vp, i64, vp, i64]
     L.capital_cholinv_factor_batched_f64.argtypes = [vp, i64, i64, vp, vp, vp, vp]
     L.capital_cholinv_solve_batched_f64.argtypes = [vp, i64, i64, vp, i64, vp, vp]
+    L.capital_cholinv_inverse_batched_f64.argtypes = [vp, i64, i64, vp, vp]
+    L.capital_cholinv_sygst_batched_f64.argtypes = [vp, i64, i64, vp, vp, vp]
+    L.capital_cholinv_sygst_ab_batched_f64.argtypes = [vp, i64, i64, vp, vp, vp]
+    L.capital_cholinv_apply_rinv_batched_f64.argtypes = [vp, i64, i64, vp, ci, i64, vp, vp]
+    L.capital_cholinv_apply_r_batched_f64.argtypes = [vp, i64, i64, vp, ci, i64, vp, vp]
     L.capital_dist_trace_cholinv_sygst_ab.argtypes = [C.POINTER(Grid), i64, C.POINTER(CholinvArgs), C.POINTER(i64), i64, C.POINTER(i64)]
     L.capital_cacqr_factor_f64.argtypes = [vp, vp, i64, i64, ci, C.POINTER(CholinvArgs), ci, vp, vp]
     L.capital_cacqr_residual_f64.argtypes = [vp, vp, i64, i64, vp, ci, vp, C.POINTER(dbl), C.POINTER(dbl)]

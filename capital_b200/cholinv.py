@@ -14,6 +14,10 @@
     X = cholinv.apply_RT(args, Y, topo)                              # R^T Y, the itype 3 back-transform
     R, Rinv, info = cholinv.factor_batched(A, topo)                  # many SPD matrices A[b] (n <= 512) at once
     X = cholinv.solve_batched(Rinv, B, topo)                         # A[b] X[b] = B[b] from the batched factors
+    Ainv = cholinv.inverse_batched(Rinv, topo)                       # A[b]^-1 from the batched factors
+    C = cholinv.sygst_batched(A2, R, Rinv, topo, itype=1)            # the batched sygst, itypes 1, 2 and 3
+    X = cholinv.apply_Rinv_batched(Rinv, Y, topo)                    # and apply_RinvT_batched, apply_R_batched(R, Z), apply_RT_batched
+    w, X, info = cholinv.eigh_batched(A2, A, topo, itype=1)          # A2[b] x = l A[b] x (scipy.linalg.eigh conventions)
 
 Outputs are packed upper-triangular local blocks (policy::cholinv::Serialize) unless serialize=False."""
 from __future__ import annotations
@@ -296,3 +300,151 @@ def solve_batched(Rinv: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
     ctx = topo.context()
     ctx.check(_lib.lib().capital_cholinv_solve_batched_f64(ctx.handle, n, b, Uc.data_ptr(), k, Bc.data_ptr(), Xc.data_ptr()))
     return Xc if B.dim() == 2 else Xc.mT.contiguous()
+
+
+def _square_batch(t, what: str, name: str, like=None):
+    """(b, n) of a (b, n, n) tensor, or ValueError; with `like` = (b, n) the shapes must agree"""
+    b, n = t.shape[0], t.shape[1]
+    if t.shape[2] != n or (like is not None and (b, n) != like):
+        want = "(b, n, n)" if like is None else f"({like[0]}, {like[1]}, {like[1]})"
+        raise ValueError(f"cholinv.{what}: {name} must have shape {want}, got {tuple(t.shape)}")
+    return b, n
+
+
+def _check_n(n: int, what: str):
+    if n > _BATCHED_MAX_N:
+        raise ValueError(f"cholinv.{what}: n = {n} > {_BATCHED_MAX_N}")
+
+
+def _check_itype(itype, what: str):
+    if isinstance(itype, bool) or itype not in (1, 2, 3):
+        raise ValueError(f"cholinv.{what}: itype must be 1, 2 or 3, got {itype!r}")
+
+
+def _check_cuda(what: str, *ts):
+    if not all(t.is_cuda for t in ts) or len({t.device for t in ts}) != 1:
+        raise ValueError(f"cholinv.{what}: every tensor must be a CUDA tensor, all on the same device")
+
+
+def inverse_batched(Rinv: torch.Tensor, topo) -> torch.Tensor:
+    """A[b]^-1 = Rinv[b] @ Rinv[b].mT (LAPACK potri) with Rinv from `factor_batched` (capital_cholinv_inverse_batched_f64).  Rinv: CUDA
+    float64 (b, n, n), 1 <= n <= 512, upper triangular in torch indexing (only that triangle is read; factor_batched's output goes in
+    without a copy).  Returns (b, n, n), exactly symmetric.  Each matrix gets the bits of `inverse` on the same factor.  Enqueued on the
+    current stream without a host synchronisation."""
+    what = "inverse_batched"
+    _check_batched(Rinv, what, "Rinv", (3,))
+    b, n = _square_batch(Rinv, what, "Rinv")
+    _check_n(n, what)
+    _check_cuda(what, Rinv)
+    Ui = Rinv.mT.contiguous()  # column-major Rinv[b]
+    out = torch.empty(b, n, n, dtype=torch.float64, device=Rinv.device)
+    ctx = topo.context()
+    ctx.check(_lib.lib().capital_cholinv_inverse_batched_f64(ctx.handle, n, b, Ui.data_ptr(), out.data_ptr()))
+    return out  # column-major and symmetric bit for bit: the buffer reads the same either way
+
+
+def sygst_batched(A: torch.Tensor, R: torch.Tensor | None, Rinv: torch.Tensor | None, topo, itype: int = 1) -> torch.Tensor:
+    """Many generalized symmetric-definite eigenproblems reduced to C[b] y = lambda y with the factors of `factor_batched(B)`,
+    B[b] = R[b].mT @ R[b] (LAPACK dsygst, upper), with the eigenvalues of the pencil:
+      itype 1: A x = lambda B x,  C = Rinv^T A Rinv (capital_cholinv_sygst_batched_f64),    back-transform x = apply_Rinv_batched(Rinv, y);
+      itype 2: A B x = lambda x,  C = R A R^T       (capital_cholinv_sygst_ab_batched_f64), back-transform x = apply_Rinv_batched(Rinv, y);
+      itype 3: B A x = lambda x,  C = R A R^T       (capital_cholinv_sygst_ab_batched_f64), back-transform x = apply_RT_batched(R, y).
+    A: CUDA float64 (b, n, n), symmetric; only its lower triangle in torch indexing (A[b, i, j], i >= j) is read, as in factor_batched.
+    itype 1 reads only Rinv, itypes 2 and 3 only R (the other may be None); only their upper triangles are read.  Returns C (b, n, n),
+    exactly symmetric, with the bits of `sygst` on the same factors.  Enqueued on the current stream without a host synchronisation."""
+    what = "sygst_batched"
+    _check_batched(A, what, "A", (3,))
+    for name, t in (("R", R), ("Rinv", Rinv)):
+        if t is not None:
+            _check_batched(t, what, name, (3,))
+    like = _square_batch(A, what, "A")
+    for name, t in (("R", R), ("Rinv", Rinv)):
+        if t is not None:
+            _square_batch(t, what, name, like)
+    b, n = like
+    _check_n(n, what)
+    _check_itype(itype, what)
+    F = Rinv if itype == 1 else R
+    if F is None:
+        raise ValueError(f"cholinv.{what}: itype {itype} reads {'Rinv' if itype == 1 else 'R'}, which is None")
+    _check_cuda(what, A, F)
+    Ac = A.contiguous()  # row-major A[b] is column-major A[b]^T: the library's upper triangle is A[b]'s lower one
+    Fc = F.mT.contiguous()
+    out = torch.empty(b, n, n, dtype=torch.float64, device=A.device)
+    ctx = topo.context()
+    fn = _lib.lib().capital_cholinv_sygst_batched_f64 if itype == 1 else _lib.lib().capital_cholinv_sygst_ab_batched_f64
+    ctx.check(fn(ctx.handle, n, b, Fc.data_ptr(), Ac.data_ptr(), out.data_ptr()))
+    return out
+
+
+def _apply_batched(F: torch.Tensor, B: torch.Tensor, topo, trans: int, what: str, fname: str, factor_r: bool) -> torch.Tensor:
+    """X[b] = op(F[b]) B[b] with F = R (factor_r) or Rinv from factor_batched: the checks and layout shared by the apply_*_batched calls"""
+    _check_batched(F, what, fname, (3,))
+    _check_batched(B, what, "B", (2, 3))
+    b, n = _square_batch(F, what, fname)
+    if B.shape[0] != b or B.shape[1] != n:
+        raise ValueError(f"cholinv.{what}: B must have shape ({b}, {n}) or ({b}, {n}, k), got {tuple(B.shape)}")
+    _check_n(n, what)
+    _check_cuda(what, F, B)
+    k = 1 if B.dim() == 2 else B.shape[2]
+    Fc = F.mT.contiguous()                                      # column-major F[b] (no copy for factor_batched's output)
+    Bc = B.contiguous() if B.dim() == 2 else B.mT.contiguous()  # column-major n x k per matrix
+    Xc = torch.empty_like(Bc)
+    ctx = topo.context()
+    fn = _lib.lib().capital_cholinv_apply_r_batched_f64 if factor_r else _lib.lib().capital_cholinv_apply_rinv_batched_f64
+    ctx.check(fn(ctx.handle, n, b, Fc.data_ptr(), trans, k, Bc.data_ptr(), Xc.data_ptr()))
+    return Xc if B.dim() == 2 else Xc.mT.contiguous()
+
+
+def apply_Rinv_batched(Rinv: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = Rinv[b] @ B[b] = R[b]^-1 B[b] (capital_cholinv_apply_rinv_batched_f64, trans = 0): the back-transform of sygst_batched for
+    itypes 1 and 2.  Rinv as for `solve_batched`; B: CUDA float64 (b, n) or (b, n, k).  Returns X with B's shape, with the bits of
+    `apply_Rinv` on the same factor.  Enqueued on the current stream; deterministic."""
+    return _apply_batched(Rinv, B, topo, 0, "apply_Rinv_batched", "Rinv", False)
+
+
+def apply_RinvT_batched(Rinv: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = Rinv[b].mT @ B[b] = R[b]^-T B[b] (trans = 1): whitening.  As apply_Rinv_batched otherwise."""
+    return _apply_batched(Rinv, B, topo, 1, "apply_RinvT_batched", "Rinv", False)
+
+
+def apply_R_batched(R: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = R[b] @ B[b] with R from `factor_batched` (capital_cholinv_apply_r_batched_f64, trans = 0); only R's upper triangle in
+    torch indexing is read.  As apply_Rinv_batched otherwise."""
+    return _apply_batched(R, B, topo, 0, "apply_R_batched", "R", True)
+
+
+def apply_RT_batched(R: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
+    """X[b] = R[b].mT @ B[b] (trans = 1): the back-transform of sygst_batched for itype 3, and samples of covariance A[b] from white
+    noise B[b].  As apply_R_batched otherwise."""
+    return _apply_batched(R, B, topo, 1, "apply_RT_batched", "R", True)
+
+
+def eigh_batched(A: torch.Tensor, B: torch.Tensor, topo, itype: int = 1):
+    """Generalized symmetric-definite eigenproblems of many small pencils, with the conventions of scipy.linalg.eigh(a, b, type=itype):
+      itype 1: A[b] x = lambda B[b] x,  itype 2: A[b] B[b] x = lambda x,  itype 3: B[b] A[b] x = lambda x.
+    A, B: CUDA float64 (b, n, n), 1 <= n <= 512, symmetric, B positive definite; only their lower triangles in torch indexing are read.
+    Returns (w, X, info): eigenvalues w (b, n) in ascending order, eigenvectors X (b, n, n) in the columns, normalised X^T B X = I for
+    itypes 1 and 2 and X^T B^-1 X = I for itype 3, and factor_batched's info (b,).  A matrix with info != 0 gets NaN in w and X and
+    leaves the others untouched; nothing raises for it.
+    The composition: factor_batched(B), sygst_batched, torch.linalg.eigh on C (the eigensolver is torch's, not this library's), then
+    apply_Rinv_batched (itypes 1, 2) or apply_RT_batched (itype 3).  torch.linalg.eigh synchronises with the host."""
+    what = "eigh_batched"
+    _check_batched(A, what, "A", (3,))
+    _check_batched(B, what, "B", (3,))
+    like = _square_batch(A, what, "A")
+    _square_batch(B, what, "B", like)
+    b, n = like
+    _check_n(n, what)
+    _check_itype(itype, what)
+    _check_cuda(what, A, B)
+    R, Rinv, info = factor_batched(B, topo)
+    C = sygst_batched(A, R, Rinv, topo, itype)
+    bad = info != 0
+    # a failed factor's C is replaced by the identity on the device (no host synchronisation), so that eigh neither raises nor spends
+    # its iterations on it; its eigenpairs are NaN below
+    C = torch.where(bad.view(b, 1, 1), torch.eye(n, dtype=torch.float64, device=C.device), C)
+    w, Y = torch.linalg.eigh(C)
+    X = apply_Rinv_batched(Rinv, Y, topo) if itype in (1, 2) else apply_RT_batched(R, Y, topo)
+    nan = float("nan")
+    return w.masked_fill(bad.view(b, 1), nan), X.masked_fill(bad.view(b, 1, 1), nan), info

@@ -862,8 +862,8 @@ capital_status_t capital_cholinv_factor_batched_f64(capital_ctx* ctx, int64_t n,
     } else {
       const LeafBatch bt{cnt, {mm, mm, mm, mm}, info + b0, cw};
       CAP_TRY(basecase_cholinv(ctx, st, (int)nb, W, nb, Rw, nb, Riw, nb, RiT, nb, &bt));
-      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Rw, nb, mm, R + b0 * nn));
-      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Riw, nb, mm, Rinv + b0 * nn));
+      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Rw, nb, mm, R + b0 * nn, n, nn));
+      CAP_TRY(triu_out_batched(ctx, st, n, cnt, Riw, nb, mm, Rinv + b0 * nn, n, nn));
     }
   }
   return CAPITAL_OK;
@@ -1107,6 +1107,176 @@ capital_status_t capital_cholinv_sygst_ab_f64(capital_ctx* ctx, int64_t n, const
     CAP_CUDA(cudaStreamSynchronize(st));
   }
   return CAPITAL_OK;
+}
+
+// ---- batched inverse, sygst and products with the factors: the single-GPU sequences above, run over a chunk of matrices ----------------
+// Every matrix lives in the workspace as the single call lays it out (ld = round_up(n, 16), n columns) at a stride of ld n, so each pass
+// and product of the single call becomes one batched launch with the same flags, k ranges and class order: every matrix gets the
+// single call's bits on the same factors.  Chunks of at most 65535 matrices whose intermediates fit BATCHED_WORKSPACE_CAP.
+
+// The arguments every batched entry point shares: non-null, n in [1, 512], batch >= 1, device pointers.
+static capital_status_t batched_args(capital_ctx* ctx, const char* what, const char* names, int64_t n, int64_t batch,
+                                     std::initializer_list<const void*> ptrs, bool extra_ok = true, const char* extra = "") {
+  bool null = false;
+  for (const void* p : ptrs) null = null || !p;
+  if (null || n < 1 || batch < 1 || !extra_ok) {
+    ctx->set_error(std::string("cholinv::") + what + ": invalid arguments (" + names + " non-null, n >= 1, batch >= 1" + extra + ")");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error(std::string("cholinv::") + what + ": n > 512 is not supported");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device(ptrs)) {
+    ctx->set_error(std::string("cholinv::") + what + ": " + names + " must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  return CAPITAL_OK;
+}
+
+// matrices per chunk when each holds `per_matrix` bytes of intermediates
+static int64_t batched_chunk(int64_t batch, int64_t per_matrix) {
+  return std::min<int64_t>({batch, 65535, (int64_t)(BATCHED_WORKSPACE_CAP / per_matrix)});
+}
+
+// The workspace of the batched inverse and sygst: `count` buffers of chunk x ld x n doubles, under the batched factor's names (the two
+// calls never run at once, so they share the memory).
+static capital_status_t batched_buffers(capital_ctx* ctx, int64_t chunk, int64_t s, int count, double** out) {
+  static const char* names[4] = {"batched_Ri", "batched_RiT", "batched_W", "batched_R"};
+  for (int i = 0; i < count; i++) CAP_TRY(ctx->workspace(names[i], (size_t)(chunk * s) * 8, (void**)&out[i]));
+  return CAPITAL_OK;
+}
+
+static GemmBatchOps batch_ops(int64_t cnt, const double* A, const double* B, int64_t ld, int64_t s) {
+  GemmBatchOps g;
+  g.batch = cnt; g.A = A; g.B = B; g.lda = g.ldb = ld; g.sa = g.sb = g.sc = s;
+  return g;
+}
+
+capital_status_t capital_cholinv_inverse_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, double* Ainv) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  CAP_TRY(batched_args(ctx, "inverse_batched", "Rinv, Ainv", n, batch, {Rinv, Ainv}));
+  const int64_t nn = n * n, ld = round_up(n, 16), s = ld * n;
+  if (overlaps(Ainv, (size_t)(batch * nn), Rinv, (size_t)(batch * nn))) {
+    ctx->set_error("cholinv::inverse_batched: Ainv must not overlap Rinv");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  const int64_t chunk = batched_chunk(batch, 3 * s * 8);
+  double* w[3];
+  CAP_TRY(batched_buffers(ctx, chunk, s, 3, w));
+  double *Ri = w[0], *RiT = w[1], *W = w[2];
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    CAP_TRY(triu_out_batched(ctx, st, n, cnt, Rinv + b0 * nn, n, nn, Ri, ld, s));
+    CAP_TRY(transpose_batched(ctx, st, n, n, cnt, Ri, ld, s, RiT, ld, s));  // Rinv^T: lower, exact zeros above the diagonal
+    CAP_TRY(gemm_tn_batched(ctx, st, n, n, n, 1.0, batch_ops(cnt, RiT, RiT, ld, s), W, ld, nullptr, 0,
+                            CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER, false));
+    CAP_TRY(sym_merge_batched(ctx, st, n, cnt, W, ld, s, Ainv + b0 * nn, n, nn));
+  }
+  return CAPITAL_OK;
+}
+
+capital_status_t capital_cholinv_sygst_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, const double* A,
+                                                   double* C) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  CAP_TRY(batched_args(ctx, "sygst_batched", "Rinv, A, C", n, batch, {Rinv, A, C}));
+  const int64_t nn = n * n, ld = round_up(n, 16), s = ld * n;
+  const size_t all = (size_t)(batch * nn);
+  if (overlaps(C, all, Rinv, all) || overlaps(C, all, A, all)) {
+    ctx->set_error("cholinv::sygst_batched: C must not overlap Rinv or A");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  const int64_t chunk = batched_chunk(batch, 4 * s * 8);
+  double* w[4];
+  CAP_TRY(batched_buffers(ctx, chunk, s, 4, w));
+  double *Ri = w[0], *UT = w[1], *V = w[2], *Cm = w[3];
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    CAP_TRY(triu_out_batched(ctx, st, n, cnt, Rinv + b0 * nn, n, nn, Ri, ld, s));
+    CAP_TRY(tril_half_batched(ctx, st, n, cnt, A + b0 * nn, n, nn, UT, ld, s));  // U^T
+    CAP_CUDA(cudaMemsetAsync(V, 0, (size_t)(cnt * s) * 8, st));
+    CAP_TRY(gemm_tn_batched(ctx, st, n, n, n, 1.0, batch_ops(cnt, UT, Ri, ld, s), V, ld, nullptr, 0,
+                            CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER, false));  // V = U Rinv
+    GemmBatchOps g = batch_ops(cnt, Ri, V, ld, s);  // Rinv^T V
+    g.ncls = 2; g.A1 = V; g.B1 = Ri;                // + V^T Rinv
+    CAP_TRY(gemm_tn_batched(ctx, st, n, n, n, 1.0, g, Cm, ld, nullptr, 0, CAPITAL_GEMM_A_UPPER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER,
+                            false));
+    CAP_TRY(sym_merge_batched(ctx, st, n, cnt, Cm, ld, s, C + b0 * nn, n, nn));
+  }
+  return CAPITAL_OK;
+}
+
+capital_status_t capital_cholinv_sygst_ab_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* R, const double* A,
+                                                      double* C) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  CAP_TRY(batched_args(ctx, "sygst_ab_batched", "R, A, C", n, batch, {R, A, C}));
+  const int64_t nn = n * n, ld = round_up(n, 16), s = ld * n;
+  const size_t all = (size_t)(batch * nn);
+  if (overlaps(C, all, R, all) || overlaps(C, all, A, all)) {
+    ctx->set_error("cholinv::sygst_ab_batched: C must not overlap R or A");
+    return CAPITAL_ERR_INVALID;
+  }
+  cudaStream_t st = ctx->stream;
+  const int64_t chunk = batched_chunk(batch, 4 * s * 8);
+  double* w[4];
+  CAP_TRY(batched_buffers(ctx, chunk, s, 4, w));
+  double *Ri = w[0], *RT = w[1], *W = w[2], *Cm = w[3];  // Ri: R, then U, then W^T (as in the single call)
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    CAP_TRY(triu_out_batched(ctx, st, n, cnt, R + b0 * nn, n, nn, Ri, ld, s));
+    CAP_TRY(transpose_batched(ctx, st, n, n, cnt, Ri, ld, s, RT, ld, s));       // R^T: lower, exact zeros above the diagonal
+    CAP_TRY(tril_half_batched(ctx, st, n, cnt, A + b0 * nn, n, nn, W, ld, s));  // U^T
+    CAP_TRY(transpose_batched(ctx, st, n, n, cnt, W, ld, s, Ri, ld, s));        // U
+    CAP_CUDA(cudaMemsetAsync(W, 0, (size_t)(cnt * s) * 8, st));
+    CAP_TRY(gemm_tn_batched(ctx, st, n, n, n, 1.0, batch_ops(cnt, RT, Ri, ld, s), W, ld, nullptr, 0,
+                            CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_UPPER | CAPITAL_GEMM_C_UPPER, false));  // W = R U
+    CAP_TRY(transpose_batched(ctx, st, n, n, cnt, W, ld, s, Ri, ld, s));        // W^T: lower, exact zeros above the diagonal
+    GemmBatchOps g = batch_ops(cnt, Ri, RT, ld, s);  // W R^T
+    g.ncls = 2; g.A1 = RT; g.B1 = Ri;                // + R W^T
+    CAP_TRY(gemm_tn_batched(ctx, st, n, n, n, 1.0, g, Cm, ld, nullptr, 0, CAPITAL_GEMM_A_LOWER | CAPITAL_GEMM_B_LOWER | CAPITAL_GEMM_C_UPPER,
+                            false));
+    CAP_TRY(sym_merge_batched(ctx, st, n, cnt, Cm, ld, s, C + b0 * nn, n, nn));
+  }
+  return CAPITAL_OK;
+}
+
+// X_b = op(U_b) B_b with U = R or Rinv: per panel of up to SOLVE_W right-hand sides, the panel of every matrix of the chunk is copied
+// into T (so X may alias B), then one batched tri_apply pass over U, as the single call's apply does.
+static capital_status_t apply_batched(capital_ctx* ctx, const char* what, const char* names, int64_t n, int64_t batch, const double* U,
+                                      int trans, int64_t nrhs, const double* B, double* X) {
+  CAP_TRY(batched_args(ctx, what, names, n, batch, {U, B, X}, nrhs >= 1 && (trans == 0 || trans == 1), ", nrhs >= 1, trans 0 or 1"));
+  cudaStream_t st = ctx->stream;
+  const int64_t nn = n * n, nbk = n * nrhs, ts = n * SOLVE_W;
+  // per matrix: the panel T and tri_apply's partials (one k chunk per 64-row block: n <= 1024), as in the batched solve
+  const int64_t chunk = batched_chunk(batch, (ts + round_up(n, 64) * SOLVE_W) * 8);
+  double* T;
+  CAP_TRY(ctx->workspace("batched_T", (size_t)(chunk * ts) * 8, (void**)&T));
+  for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
+    const int64_t cnt = std::min(chunk, batch - b0);
+    const double* Ub = U + b0 * nn;
+    for (int64_t p0 = 0; p0 < nrhs; p0 += SOLVE_W) {
+      const int64_t w = std::min<int64_t>(SOLVE_W, nrhs - p0);
+      CAP_TRY(copy_batched(ctx, st, n, w, cnt, B + b0 * nbk + p0 * n, n, nbk, T, n, ts));
+      //                 U   ldu trans  r0 r1 c0 c1 nrhs alpha P  pinc ldp beta Cin   ldcin C                       cinc ldc full  batch su  sp  scin sc
+      CAP_TRY(tri_apply(ctx, st, {Ub, n, trans == 1, 0, n, 0, n, w, 1.0, T, 1, n, 0.0, nullptr, 0, X + b0 * nbk + p0 * n, 1, n, false, cnt, nn, ts, 0, nbk}));
+    }
+  }
+  return CAPITAL_OK;
+}
+
+capital_status_t capital_cholinv_apply_rinv_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, int trans,
+                                                        int64_t nrhs, const double* B, double* X) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  return apply_batched(ctx, "apply_rinv_batched", "Rinv, B, X", n, batch, Rinv, trans, nrhs, B, X);
+}
+
+capital_status_t capital_cholinv_apply_r_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* R, int trans, int64_t nrhs,
+                                                     const double* B, double* X) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  return apply_batched(ctx, "apply_r_batched", "R, B, X", n, batch, R, trans, nrhs, B, X);
 }
 
 // ||A Ainv - I||_F / ||I||_F (the inverse validator of the reference, test/inverse/validate.hpp:7-34, with the diagonal taken by global

@@ -150,7 +150,8 @@ capital_status_t gemm_tn_t(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t
 // split-k chunk count of gemm_tn_splitk for this shape (and whether it runs 128 x 128 tiles)
 int64_t gemm_splitk_chunks(const capital_ctx* ctx, int64_t m, int64_t n, int64_t k, int flags, bool* big);
 // A batch of products of one shape: matrix b reads A + b sa and B + b sb (16-byte aligned bases, even lda, ldb, sa, sb) and writes
-// C + b sc, Ct + b sct (gemm_tn_batched, gemm_tn.cu)
+// C + b sc, Ct + b sct (gemm_tn_batched, gemm_tn.cu).  ncls = 2 adds a second operand class (A1, B1: the same lda, ldb, sa, sb),
+// summed after class 0 in the same launch as gemm_tn_x does; beta != 0 adds beta C_b (read at C + b sc).
 struct GemmBatchOps {
   int64_t batch = 1;
   const double* A = nullptr;
@@ -158,6 +159,10 @@ struct GemmBatchOps {
   const double* B = nullptr;
   int64_t ldb = 0, sb = 0;
   int64_t sc = 0, sct = 0;
+  int ncls = 1;
+  const double* A1 = nullptr;
+  const double* B1 = nullptr;
+  double beta = 0.0;
 };
 capital_status_t gemm_tn_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmBatchOps& b,
                                  double* C, int64_t ldc, double* Ct, int64_t ldct, int flags, bool gram);
@@ -196,11 +201,20 @@ capital_status_t sym_merge(capital_ctx* ctx, cudaStream_t st, int64_t n, const d
 capital_status_t tril_half_copy(capital_ctx* ctx, cudaStream_t st, int64_t n, const double* src, int64_t lds, double* dst, int64_t ldd,
                                 int x, int y, int d);
 // Batched factor (n <= BASECASE_MAX): W_b, nb x nb (nb a multiple of 32), from the upper triangle of A_b (n x n contiguous, mirrored below
-// the diagonal; the lower triangle is never read), the identity in the pad; and back: dst_b (n x n contiguous) = triu of the leading
+// the diagonal; the lower triangle is never read), the identity in the pad; and back: dst_b (ld ldd, stride sd) = triu of the leading
 // n x n block of src_b (ld lds, stride ss), exact zeros below the diagonal.
 capital_status_t sym_pad_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t nb, int64_t batch, const double* A, double* W);
 capital_status_t triu_out_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
-                                  double* dst);
+                                  double* dst, int64_t ldd, int64_t sd);
+// Batched inverse / sygst (matrix b at src + b ss, dst + b sd, <= 65535 matrices): tril_half_copy's operand U_b^T (diagonal halved,
+// zeros above), read from A_b's UPPER triangle; sym_merge on one GPU (out_b from the upper triangle of U_b and its mirror; <= 65535 matrices); and a plain copy
+// of rows x cols blocks (the right-hand-side panels of the batched products).
+capital_status_t tril_half_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
+                                   double* dst, int64_t ldd, int64_t sd);
+capital_status_t sym_merge_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* U, int64_t ldu, int64_t su,
+                                   double* out, int64_t ldo, int64_t so);
+capital_status_t copy_batched(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, int64_t batch, const double* src, int64_t lds,
+                              int64_t ss, double* dst, int64_t ldd, int64_t sd);
 capital_status_t gen_symmetric(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,
                                int64_t n_global, int x, int y, int d, int diag_dom);
 capital_status_t gen_random(capital_ctx* ctx, cudaStream_t st, double* A, int64_t ld, int64_t lrows, int64_t lcols,

@@ -2540,7 +2540,7 @@ capital_status_t dist_cacqr_factor_batched(capital_ctx* ctx, int64_t m, int64_t 
     } else {
       CAP_TRY(sweep_batched(q, Qc, ldqc, sqc, q.Qt, nullptr, Qb, m, mn, R1));
     }
-    CAP_TRY(triu_out_batched(ctx, st, n, q.cnt, Rfinal, q.nr, rr, R + b0 * n * n));
+    CAP_TRY(triu_out_batched(ctx, st, n, q.cnt, Rfinal, q.nr, rr, R + b0 * n * n, n, n * n));
   }
   return CAPITAL_OK;
 }

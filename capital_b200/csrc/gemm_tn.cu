@@ -403,13 +403,17 @@ capital_status_t launch_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, in
   constexpr int BM = Cfg::BM, BN = Cfg::BN;
   GemmParams p{};
   p.Ct = ex.Ct; p.ldct = ex.ldct; p.no_c = ex.no_c; p.kpart = ex.kpart; p.kstride = ex.kstride; p.ldk = ex.ldk;
-  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = 0.0; p.C = C; p.ldc = ldc; p.ksplit = ksplit;
-  p.ncls = 1;
+  p.M = (int)m; p.N = (int)n; p.K = (int)k; p.flags = flags; p.alpha = alpha; p.beta = b.beta; p.C = C; p.ldc = ldc; p.ksplit = ksplit;
+  p.ncls = b.ncls;
   p.sc = b.sc; p.sct = b.sct; p.skp = skp;
   GemmMaps maps;
   memset(&maps, 0, sizeof(maps));
   CAP_TRY(make_map_3d(ctx, &maps.a[0], b.A, k, m, b.lda, b.sa, b.batch, BK, BM));
   CAP_TRY(make_map_3d(ctx, &maps.b[0], b.B, k, n, b.ldb, b.sb, b.batch, BK, BN));
+  if (b.ncls == 2) {
+    CAP_TRY(make_map_3d(ctx, &maps.a[1], b.A1, k, m, b.lda, b.sa, b.batch, BK, BM));
+    CAP_TRY(make_map_3d(ctx, &maps.b[1], b.B1, k, n, b.ldb, b.sb, b.batch, BK, BN));
+  }
   p.gm = (int)ceil_div(m, BM); p.gn = (int)ceil_div(n, BN);
   const int64_t piece = 65535 / ksplit;
   for (int64_t b0 = 0; b0 < b.batch; b0 += piece) {
@@ -550,15 +554,19 @@ capital_status_t gemm_tn_splitk(capital_ctx* ctx, cudaStream_t st, int64_t m, in
 // and tile of gemm_tn_splitk (gemm_splitk_chunks) and its two-stage reduction; otherwise one chunk, alpha A^T B stored into C (ldc
 // >= m, stride sc; C may be nullptr when only Ct is wanted) and, when Ct is set, transposed into Ct (ldct, stride sct) as gemm_tn_t
 // does.  Every matrix gets the bits of the single product of the same shape and flags: the tile may differ from the single
-// product's only where the extra k tiles of a triangular operand add exact zeros.
+// product's only where the extra k tiles of a triangular operand add exact zeros.  Two operand classes (b.ncls = 2) and beta run as
+// in gemm_tn_x, class 0's k tiles first; the Gram product takes neither.
 capital_status_t gemm_tn_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, int64_t n, int64_t k, double alpha, const GemmBatchOps& b,
                                  double* C, int64_t ldc, double* Ct, int64_t ldct, int flags, bool gram) {
   if (m <= 0 || n <= 0 || k <= 0 || b.batch <= 0) return CAPITAL_OK;
+  const bool two = b.ncls == 2;
   const bool bad = b.lda < k || b.ldb < k || (b.lda & 1) || (b.ldb & 1) || (b.sa & 1) || (b.sb & 1) || (((uintptr_t)b.A | (uintptr_t)b.B) & 15) ||
                    (C && ldc < m) || (!C && !Ct) || (Ct && ldct < n) || (gram && (Ct || !C)) || m >= (1LL << 31) || n >= (1LL << 31) ||
-                   k >= (1LL << 31) - 16;
+                   k >= (1LL << 31) - 16 || (b.ncls != 1 && !two) || (two && (!b.A1 || !b.B1 || (((uintptr_t)b.A1 | (uintptr_t)b.B1) & 15))) ||
+                   (b.beta != 0.0 && !C) || (gram && (two || b.beta != 0.0));
   if (bad) {
-    ctx->set_error("gemm_tn_batched: invalid operands (16-byte aligned, even leading dimensions and strides, lda, ldb >= k)");
+    ctx->set_error("gemm_tn_batched: invalid operands (16-byte aligned, even leading dimensions and strides, lda, ldb >= k; one or two "
+                   "operand classes; the Gram product takes one class and beta = 0)");
     return CAPITAL_ERR_INVALID;
   }
   ctx->counters.gemm_launches++;
@@ -568,6 +576,7 @@ capital_status_t gemm_tn_batched(capital_ctx* ctx, cudaStream_t st, int64_t m, i
   else if (atri) f = (double)n * (double)m * (double)(m + 1);
   else if (btri) f = (double)m * (double)n * (double)(n + 1);
   else if (flags & CAPITAL_GEMM_C_UPPER) f = (double)k * (double)m * (double)(m + 1);
+  f *= b.ncls;
   ctx->counters.gemm_flops += f * (double)b.batch;
   GemmExtra ex;
   ex.Ct = Ct; ex.ldct = ldct; ex.no_c = C ? 0 : 1;

@@ -139,13 +139,68 @@ __global__ void sym_pad_batched_kernel(int n, int nb, const double* A, double* W
   }
 }
 
-// Copy-out of the batched factor: dst_b (n x n, ld n, at dst + b n n) = the upper triangle of the leading n x n block of src_b (ld lds,
-// at src + b ss), exact zeros below the diagonal.
-__global__ void triu_out_batched_kernel(long long n, long long batch, const double* src, long long lds, long long ss, double* dst) {
+// dst_b (n x n, ld ldd, at dst + b sd) = the upper triangle of the leading n x n block of src_b (ld lds, at src + b ss), exact zeros
+// below the diagonal; src's strictly lower triangle is never read.  The copy-out of the batched factor, and the copy-in of a factor
+// into the ld-padded workspace of the batched inverse, sygst and products.
+__global__ void triu_out_batched_kernel(long long n, long long batch, const double* src, long long lds, long long ss, double* dst,
+                                        long long ldd, long long sd) {
   const long long nn = n * n, total = nn * batch;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long b = i / nn, e = i - b * nn, c = e / n, r = e - c * n;
-    dst[i] = r <= c ? src[b * ss + c * lds + r] : 0.0;
+    dst[b * sd + c * ldd + r] = r <= c ? src[b * ss + c * lds + r] : 0.0;
+  }
+}
+
+// The operand U^T of the batched sygst on matrix blockIdx.z: dst_b (ld ldd, at dst + b sd) = U_b^T with U_b = triu(A_b), its diagonal
+// halved, zeros above U^T's diagonal -- tril_half_copy's operand on one GPU, but read from A_b's UPPER triangle (n x n, ld lds, at
+// src + b ss; the triangle the batched factor reads), which for a symmetric A holds the same values.  A's strict lower triangle is never
+// read.  A transpose of 32 x 32 tiles through shared memory, so that the reads and the writes stay coalesced.
+__global__ void tril_half_batched_kernel(int n, const double* src, long long lds, long long ss, double* dst, long long ldd, long long sd) {
+  __shared__ double tile[TP][TP + 1];
+  src += (long long)blockIdx.z * ss;
+  dst += (long long)blockIdx.z * sd;
+  const int r0 = blockIdx.x * TP, c0 = blockIdx.y * TP;
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int r = r0 + threadIdx.x, c = c0 + j;
+    if (r < n && c < n) tile[j][threadIdx.x] = r < c ? src[(long long)c * lds + r] : (r == c ? 0.5 * src[(long long)c * lds + r] : 0.0);
+  }
+  __syncthreads();
+  // dst(c, r) = U(r, c)
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int c = c0 + threadIdx.x, r = r0 + j;
+    if (r < n && c < n) dst[(long long)r * ldd + c] = tile[threadIdx.x][j];
+  }
+}
+
+// sym_merge_kernel (one GPU: S = U read transposed) on matrix blockIdx.z of a batch: out_b(r, c) = U_b(r, c) for r <= c, U_b(c, r)
+// below the diagonal.  Only U's upper triangle reaches the output.
+__global__ void sym_merge_batched_kernel(int n, const double* U, long long ldu, long long su, double* out, long long ldo, long long so) {
+  __shared__ double tile[TP][TP + 1];
+  U += (long long)blockIdx.z * su;
+  out += (long long)blockIdx.z * so;
+  const int r0 = blockIdx.x * TP, c0 = blockIdx.y * TP;
+  const bool all_upper = r0 + TP - 1 <= c0;
+  if (!all_upper) {
+    for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+      const int r = r0 + j, c = c0 + threadIdx.x;
+      if (r < n && c < n) tile[j][threadIdx.x] = U[(long long)r * ldu + c];  // U(c, r)
+    }
+    __syncthreads();
+  }
+  for (int j = threadIdx.y; j < TP; j += blockDim.y) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    if (r >= n || c >= n) continue;
+    out[(long long)c * ldo + r] = r <= c ? U[(long long)c * ldu + r] : tile[threadIdx.x][j];
+  }
+}
+
+// dst_b (rows x cols, ld ldd, at dst + b sd) = src_b (ld lds, at src + b ss): the right-hand-side panels of the batched products
+__global__ void copy_batched_kernel(long long rows, long long cols, long long batch, const double* src, long long lds, long long ss,
+                                    double* dst, long long ldd, long long sd) {
+  const long long per = rows * cols, total = per * batch;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / per, e = i - b * per, c = e / rows, r = e - c * rows;
+    dst[b * sd + c * ldd + r] = src[b * ss + c * lds + r];
   }
 }
 
@@ -406,9 +461,34 @@ capital_status_t sym_pad_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, i
   return CAPITAL_OK;
 }
 capital_status_t triu_out_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
-                                  double* dst) {
+                                  double* dst, int64_t ldd, int64_t sd) {
   if (n <= 0 || batch <= 0) return CAPITAL_OK;
-  triu_out_batched_kernel<<<grid_for(ctx, n * n * batch, 256), 256, 0, st>>>(n, batch, src, lds, ss, dst);
+  triu_out_batched_kernel<<<grid_for(ctx, n * n * batch, 256), 256, 0, st>>>(n, batch, src, lds, ss, dst, ldd, sd);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t tril_half_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* src, int64_t lds, int64_t ss,
+                                   double* dst, int64_t ldd, int64_t sd) {
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  if (batch > 65535) return CAPITAL_ERR_INVALID;
+  dim3 grid((unsigned)ceil_div(n, TP), (unsigned)ceil_div(n, TP), (unsigned)batch), block(TP, 8);
+  tril_half_batched_kernel<<<grid, block, 0, st>>>((int)n, src, lds, ss, dst, ldd, sd);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t sym_merge_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* U, int64_t ldu, int64_t su,
+                                   double* out, int64_t ldo, int64_t so) {
+  if (n <= 0 || batch <= 0) return CAPITAL_OK;
+  if (batch > 65535) return CAPITAL_ERR_INVALID;
+  dim3 grid((unsigned)ceil_div(n, TP), (unsigned)ceil_div(n, TP), (unsigned)batch), block(TP, 8);
+  sym_merge_batched_kernel<<<grid, block, 0, st>>>((int)n, U, ldu, su, out, ldo, so);
+  LAUNCH_CHECK();
+  return CAPITAL_OK;
+}
+capital_status_t copy_batched(capital_ctx* ctx, cudaStream_t st, int64_t rows, int64_t cols, int64_t batch, const double* src, int64_t lds,
+                              int64_t ss, double* dst, int64_t ldd, int64_t sd) {
+  if (rows <= 0 || cols <= 0 || batch <= 0) return CAPITAL_OK;
+  copy_batched_kernel<<<grid_for(ctx, rows * cols * batch, 256), 256, 0, st>>>(rows, cols, batch, src, lds, ss, dst, ldd, sd);
   LAUNCH_CHECK();
   return CAPITAL_OK;
 }

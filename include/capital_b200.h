@@ -215,6 +215,30 @@ capital_status_t capital_cholinv_factor_batched_f64(capital_ctx* ctx, int64_t n,
  * stream.  Errors as capital_cholinv_factor_batched_f64 (nrhs < 1: CAPITAL_ERR_INVALID). */
 capital_status_t capital_cholinv_solve_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, int64_t nrhs,
                                                    const double* B, double* X);
+/* The batched inverse, sygst and products with the factors: for each of `batch` matrices of order 1 <= n <= 512 the single-GPU call of
+ * the same name (capital_cholinv_inverse_f64, _sygst_f64, _sygst_ab_f64, _apply_rinv_f64, _apply_r_f64), on the outputs of
+ * capital_cholinv_factor_batched_f64, with that call's bits on the same factors.  All matrices column-major, matrix b at offset b n n
+ * (b n nrhs for B and X).  R and Rinv are read as the batched factor wrote them, and only their upper triangles: whatever lies below
+ * the diagonal changes no bit.  Of A only the upper triangle of each A_b, the diagonal included, is read (the triangle the batched
+ * factor reads).  C and Ainv are written whole, exactly symmetric: the lower half is the upper half's mirror, bit for bit; they must
+ * not overlap any input (CAPITAL_ERR_INVALID).  X may alias B.  Device pointers only; enqueued on the context stream with no host
+ * synchronisation; never communicates, so on a grid context each rank works on its own batch.  Intermediates take at most 2 GiB of
+ * device memory (kept until capital_release_workspace): larger batches run in chunks of at most 65535 matrices.  n > 512:
+ * CAPITAL_ERR_UNSUPPORTED; n < 1, batch < 1, nrhs < 1, trans not 0 or 1, a NULL argument or a host pointer: CAPITAL_ERR_INVALID. */
+/* Ainv_b = Rinv_b Rinv_b^T = A_b^-1 (LAPACK potri): one DMMA product of n^3 / 3 flops per matrix. */
+capital_status_t capital_cholinv_inverse_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, double* Ainv);
+/* itype 1: C_b = Rinv_b^T A_b Rinv_b (A x = lambda B x), n^3 flops per matrix. */
+capital_status_t capital_cholinv_sygst_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, const double* A,
+                                                   double* C);
+/* itype 2 and 3: C_b = R_b A_b R_b^T (A B x = lambda x, B A x = lambda x), n^3 flops per matrix. */
+capital_status_t capital_cholinv_sygst_ab_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* R, const double* A,
+                                                      double* C);
+/* trans 0: X_b = Rinv_b B_b (the back-transform of itype 1 and 2); trans 1: X_b = Rinv_b^T B_b (whitening). */
+capital_status_t capital_cholinv_apply_rinv_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* Rinv, int trans,
+                                                        int64_t nrhs, const double* B, double* X);
+/* trans 0: X_b = R_b B_b; trans 1: X_b = R_b^T B_b (the back-transform of itype 3; samples of covariance A_b from white noise). */
+capital_status_t capital_cholinv_apply_r_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* R, int trans,
+                                                     int64_t nrhs, const double* B, double* X);
 
 /* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
  * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
