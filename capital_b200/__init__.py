@@ -5,6 +5,6 @@ product is the C-ABI shared library (include/capital_b200.h) built from capital_
 from . import _lib
 from . import topology as topo
 from .matrix import matrix
-from . import cholinv, cacqr, summa
+from . import cholinv, cacqr, summa, eig
 
-__all__ = ["topo", "matrix", "cholinv", "cacqr", "summa", "_lib"]
+__all__ = ["topo", "matrix", "cholinv", "cacqr", "summa", "eig", "_lib"]

@@ -420,15 +420,18 @@ def apply_RT_batched(R: torch.Tensor, B: torch.Tensor, topo) -> torch.Tensor:
     return _apply_batched(R, B, topo, 1, "apply_RT_batched", "R", True)
 
 
-def eigh_batched(A: torch.Tensor, B: torch.Tensor, topo, itype: int = 1):
+def eigh_batched(A: torch.Tensor, B: torch.Tensor, topo, itype: int = 1, eigensolver: str = "torch"):
     """Generalized symmetric-definite eigenproblems of many small pencils, with the conventions of scipy.linalg.eigh(a, b, type=itype):
       itype 1: A[b] x = lambda B[b] x,  itype 2: A[b] B[b] x = lambda x,  itype 3: B[b] A[b] x = lambda x.
     A, B: CUDA float64 (b, n, n), 1 <= n <= 512, symmetric, B positive definite; only their lower triangles in torch indexing are read.
     Returns (w, X, info): eigenvalues w (b, n) in ascending order, eigenvectors X (b, n, n) in the columns, normalised X^T B X = I for
     itypes 1 and 2 and X^T B^-1 X = I for itype 3, and factor_batched's info (b,).  A matrix with info != 0 gets NaN in w and X and
     leaves the others untouched; nothing raises for it.
-    The composition: factor_batched(B), sygst_batched, torch.linalg.eigh on C (the eigensolver is torch's, not this library's), then
-    apply_Rinv_batched (itypes 1, 2) or apply_RT_batched (itype 3).  torch.linalg.eigh synchronises with the host."""
+    The composition: factor_batched(B), sygst_batched, an eigensolver on C, then apply_Rinv_batched (itypes 1, 2) or apply_RT_batched
+    (itype 3).  eigensolver="torch" (the default) runs torch.linalg.eigh on C, which synchronises with the host; "jacobi" runs this
+    library's eig.syevj_batched, and a matrix whose factor succeeded but whose Jacobi iteration did not converge (or whose A holds NaN
+    or Inf) then gets info = n + 1, with NaN in w and X as for a failed factor (a failed pivot is at most n, so the two never collide).
+    The two solvers agree to rounding, up to the signs of the eigenvectors."""
     what = "eigh_batched"
     _check_batched(A, what, "A", (3,))
     _check_batched(B, what, "B", (3,))
@@ -437,6 +440,8 @@ def eigh_batched(A: torch.Tensor, B: torch.Tensor, topo, itype: int = 1):
     b, n = like
     _check_n(n, what)
     _check_itype(itype, what)
+    if not isinstance(eigensolver, str) or eigensolver not in ("torch", "jacobi"):
+        raise ValueError(f"cholinv.{what}: eigensolver must be 'torch' or 'jacobi', got {eigensolver!r}")
     _check_cuda(what, A, B)
     R, Rinv, info = factor_batched(B, topo)
     C = sygst_batched(A, R, Rinv, topo, itype)
@@ -444,7 +449,13 @@ def eigh_batched(A: torch.Tensor, B: torch.Tensor, topo, itype: int = 1):
     # a failed factor's C is replaced by the identity on the device (no host synchronisation), so that eigh neither raises nor spends
     # its iterations on it; its eigenpairs are NaN below
     C = torch.where(bad.view(b, 1, 1), torch.eye(n, dtype=torch.float64, device=C.device), C)
-    w, Y = torch.linalg.eigh(C)
+    if eigensolver == "jacobi":
+        from .eig import syevj_batched
+        w, Y, einfo = syevj_batched(C, topo)
+        info = torch.where(bad | (einfo == 0), info, torch.full_like(info, n + 1))
+        bad = info != 0
+    else:
+        w, Y = torch.linalg.eigh(C)
     X = apply_Rinv_batched(Rinv, Y, topo) if itype in (1, 2) else apply_RT_batched(R, Y, topo)
     nan = float("nan")
     return w.masked_fill(bad.view(b, 1), nan), X.masked_fill(bad.view(b, 1, 1), nan), info

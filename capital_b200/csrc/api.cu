@@ -370,7 +370,7 @@ capital_status_t capital_create(capital_ctx** out, const capital_grid_t* grid, i
   ok = ok && cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) == cudaSuccess && fn != nullptr;
   if (!ok) { capital_destroy(ctx); return CAPITAL_ERR_CUDA; }
   ctx->encode = (cuTensorMapEncodeTiled_fn)fn;
-  if (gemm_tn_init(ctx) != CAPITAL_OK || leaf_init(ctx) != CAPITAL_OK) { capital_destroy(ctx); return CAPITAL_ERR_CUDA; }
+  if (gemm_tn_init(ctx) != CAPITAL_OK || leaf_init(ctx) != CAPITAL_OK || syevj_init(ctx) != CAPITAL_OK) { capital_destroy(ctx); return CAPITAL_ERR_CUDA; }
   if (const char* e = getenv("CAPITAL_TF32_MIN_K")) ctx->tf32_min_k = atoll(e);
   if (const char* e = getenv("CAPITAL_FAR_MIN")) ctx->far_min = atoll(e);
   if (const char* e = getenv("CAPITAL_SIDE_MIN")) ctx->side_min = atoll(e);
@@ -804,8 +804,6 @@ capital_status_t capital_cholinv_apply_r_f64(capital_ctx* ctx, int64_t n, const 
 }
 
 // ---- batched CholInv: many independent n x n matrices, n <= BASECASE_MAX, on this context's GPU ------------------------------------
-// Device memory the batched factor and solve hold for intermediates, whatever the batch: larger batches run in chunks.
-constexpr size_t BATCHED_WORKSPACE_CAP = size_t(2) << 30;
 
 static bool all_device(std::initializer_list<const void*> ptrs) {
   for (const void* p : ptrs)
@@ -1241,6 +1239,32 @@ capital_status_t capital_cholinv_sygst_ab_batched_f64(capital_ctx* ctx, int64_t 
     CAP_TRY(sym_merge_batched(ctx, st, n, cnt, Cm, ld, s, C + b0 * nn, n, nn));
   }
   return CAPITAL_OK;
+}
+
+// ---- batched symmetric eigensolver (syevj.cu) ---------------------------------------------------------------------------------------
+capital_status_t capital_syevj_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* A, double* w, double* V, int* info) {
+  if (!ctx) return CAPITAL_ERR_INVALID;
+  if (!A || !w || !V || !info || n < 1 || batch < 1) {
+    ctx->set_error("syevj_batched: invalid arguments (A, w, V, info non-null, n >= 1, batch >= 1)");
+    return CAPITAL_ERR_INVALID;
+  }
+  if (n > BASECASE_MAX) {
+    ctx->set_error("syevj_batched: n > 512 is not supported");
+    return CAPITAL_ERR_UNSUPPORTED;
+  }
+  CAP_CUDA(cudaSetDevice(ctx->device));
+  if (!all_device({A, w, V, info})) {
+    ctx->set_error("syevj_batched: A, w, V and info must be device pointers");
+    return CAPITAL_ERR_INVALID;
+  }
+  const size_t nn = (size_t)(batch * n * n), nw = (size_t)(batch * n);
+  if (overlaps(w, nw, A, nn) || overlaps(V, nn, A, nn) || overlaps(w, nw, V, nn) ||
+      overlaps((const double*)info, ((size_t)batch + 1) / 2, A, nn) || overlaps((const double*)info, ((size_t)batch + 1) / 2, w, nw) ||
+      overlaps((const double*)info, ((size_t)batch + 1) / 2, V, nn)) {
+    ctx->set_error("syevj_batched: w, V and info must not overlap each other or A");
+    return CAPITAL_ERR_INVALID;
+  }
+  return syevj_batched(ctx, ctx->stream, n, batch, A, w, V, info);
 }
 
 // X_b = op(U_b) B_b with U = R or Rinv: per panel of up to SOLVE_W right-hand sides, the panel of every matrix of the chunk is copied

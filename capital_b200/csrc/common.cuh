@@ -266,6 +266,17 @@ static inline int batched_cluster_width(int64_t nb) {
   return T <= 2 ? 2 : T <= 4 ? 4 : 8;
 }
 
+// Device memory the batched calls hold for intermediates, whatever the batch: larger batches run in chunks.
+constexpr size_t BATCHED_WORKSPACE_CAP = size_t(2) << 30;
+
+// ---- syevj.cu ---------------------------------------------------------------------------------
+// Batched symmetric eigensolver (capital_syevj_batched_f64), arguments already checked: n <= BASECASE_MAX, device pointers.
+capital_status_t syevj_init(capital_ctx* ctx);  // per-device kernel attributes
+// matrices per chunk: at most 65535, and for n > 64 as many as fit BATCHED_WORKSPACE_CAP
+int64_t syevj_chunk(int64_t n, int64_t batch);
+capital_status_t syevj_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int64_t batch, const double* A, double* w, double* V,
+                               int* info);
+
 // ---- cholinv.cu -------------------------------------------------------------------------------
 // local (single-GPU) recursive CholInv on dense n x n blocks; W is destroyed (Schur complements).
 // Optional callbacks of the top-level call (cholinv::factor on one GPU): `need_cols` makes the chain's stream `st` wait until

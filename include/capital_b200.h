@@ -240,6 +240,21 @@ capital_status_t capital_cholinv_apply_rinv_batched_f64(capital_ctx* ctx, int64_
 capital_status_t capital_cholinv_apply_r_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* R, int trans,
                                                      int64_t nrhs, const double* B, double* X);
 
+/* Batched symmetric eigensolver on this context's GPU: A_b = V_b diag(w_b) V_b^T for `batch` symmetric matrices of order 1 <= n <= 512,
+ * by parallel cyclic Jacobi (one CTA per matrix for n <= 64, block Jacobi on 64 x 64 DMMA tile products above).  A, V: batch x n x n,
+ * column-major, matrix b at offset b n n; w: batch x n.  Only the upper triangle of each A_b, the diagonal included, is read (the
+ * triangle capital_cholinv_factor_batched_f64 reads); the other may hold anything, NaN included.  w_b holds the eigenvalues in
+ * ascending order and column j of V_b the eigenvector of w_b[j].  info[b] = 0 when A_b converged, 1 when it did not within the fixed
+ * sweep bound (w_b and V_b then hold the last iterate); a matrix containing NaN or Inf gets info = 1 and unspecified outputs, and
+ * never affects the others.  Each matrix gets the same bits whatever batch or chunk it is in, from run to run.
+ * Host synchronisation: for n > 64 the call reads one device counter per outer sweep (and so returns when the work is done) to stop
+ * once every matrix has converged; that is its only synchronisation.  For n <= 64 it is enqueued on the context stream with none.
+ * Device pointers only; w, V and info must not overlap each other or A.  Intermediates (n > 64) take at most 2 GiB of device memory
+ * (kept until capital_release_workspace): larger batches run in chunks of at most 65535 matrices.  n > 512: CAPITAL_ERR_UNSUPPORTED;
+ * n < 1, batch < 1, a NULL argument, a host pointer or overlapping outputs: CAPITAL_ERR_INVALID. */
+capital_status_t capital_syevj_batched_f64(capital_ctx* ctx, int64_t n, int64_t batch, const double* A, double* w, double* V,
+                                           int* info);
+
 /* cholesky::cholinv inverse: A^-1 = Rinv Rinv^T from the outputs of capital_cholinv_factor_f64 (LAPACK potri).  Collective on a grid:
  * every rank calls it with the same n_global, args (the ones given to the factor) and structure.  R_local / Rinv_local: this rank's
  * local blocks exactly as the factor wrote them; R_local is read only when the top-level Rinv12 block was skipped (complete_inv = 0
