@@ -8,13 +8,21 @@
 //             V[:, P] <- V[:, P] Q_P run as 64 x 64 x 64 DMMA tile products (syevj_update_kernel).  A matrix has converged after an
 //             outer sweep in which no subproblem rotated; its CTAs exit at once from then on.  The host reads one counter per sweep.
 //
-// Threshold: rotation (p, q) is skipped iff |a_pq| <= max(u sqrt|a_pp| sqrt|a_qq|, u ||A||_F), u = 2^-53, ||A||_F of the input.
+// Scaling: every matrix is solved as A^ = 4^-s A, s = floor(e / 2) and e = ilogb max |a_ij|, so A^'s largest entry lies in [1, 4);
+// w = 4^s w^ at the end (ldexp), V as computed.  Neither ||A^||_F nor tau = (a_qq - a_pp) / (2 a_pq) can overflow, and neither the
+// floor nor the threshold below can underflow, whatever A's magnitude: a finite A whose ||A||_F exceeds DBL_MAX is solved, and so is
+// one near the bottom of the range (otherwise every rotation there would round at the subnormal spacing).  Entries more than about
+// 2^1074 below the largest flush to zero on the scale-down; they are far below the floor.  An eigenvalue beyond DBL_MAX comes back as
+// +-Inf with info = 0 and its V.  Only a NaN or Inf entry makes a matrix non-finite (info = 1, NaN outputs).
+//
+// Threshold: rotation (p, q) is skipped iff |a_pq| <= max(u sqrt|a_pp| sqrt|a_qq|, u ||A^||_F), u = 2^-53, ||A^||_F of the input.
 // The first term is the Demmel-Veselic relative criterion.  The floor keeps singular and graded matrices from rotating forever:
 // every rotation of a row holding an O(||A||) entry leaves rounding noise of order u ||A|| in its other entries, so a floor below
 // that level (u ||A||_F / n was tried) chases noise, and graded matrices (eigenvalues 1e-15 .. 1) at n = 512 did not converge in 30
 // sweeps.  Dropping the entries below the floor moves an eigenvalue by at most ||E||_2 <= ||E||_F <= n u ||A||_F.  Every formula is exact under a
 // scaling of A by 4^k (sqrt|a_pp| sqrt|a_qq| rather than sqrt|a_pp a_qq|, a norm summed at the scale of the largest entry), so a
-// matrix scaled by 4^k gets 2^2k times the bits of the unscaled one as long as nothing underflows.
+// matrix scaled by 4^k gets 2^2k times the bits of the unscaled one as long as nothing underflows; that is why the normalisation
+// above changes no bit of a matrix whose own run neither overflows nor underflows, and why it uses powers of 4.
 //
 // Padding: pad rows and columns are exactly zero off the diagonal (zero on it), so every rotation that would couple a pad index with
 // a real one sees a_pq = 0 and is skipped, and every product keeps those couplings exactly zero.  The finish drops pad indices by
@@ -52,10 +60,12 @@ __device__ __forceinline__ void circle_pair(int m, int s, int k, int& p, int& q)
   p = min(a, b); q = max(a, b);
 }
 
-// ||M||_F of the m x m matrix get(i, j), summed at the scale 2^e of its largest entry (exact under power-of-two scaling), in a fixed
-// order (deterministic).  +Inf when an entry is NaN or infinite.  All JT threads call; red: JT doubles of shared scratch.
+// ||M||_F of the m x m matrix get(i, j) as ldexp(r, e): e = ilogb of its largest |entry|, r the norm summed at the scale 2^-e (exact
+// under power-of-two scaling, and finite whatever the entries' magnitude), in a fixed order (deterministic).  A zero matrix gives
+// r = 0, e = 0.  Returns false, with r = 0 and e = 0, when an entry is NaN or infinite.  All JT threads call; red: JT doubles of
+// shared scratch.
 template <class Get>
-__device__ double block_fro(int m, Get get, double* red) {
+__device__ bool block_fro(int m, Get get, double* red, double& r, int& e) {
   const int tid = threadIdx.x, mm = m * m;
   double mx = 0.0;
   int bad = 0;
@@ -73,13 +83,14 @@ __device__ double block_fro(int m, Get get, double* red) {
   }
   mx = red[0];
   __syncthreads();
-  if (bad) return INFINITY;
-  if (mx == 0.0) return 0.0;
-  const int e = ilogb(mx);
-  const double sc = ldexp(1.0, -e);
+  r = 0.0;
+  e = 0;
+  if (bad) return false;
+  if (mx == 0.0) return true;
+  e = ilogb(mx);
   double s = 0.0;
   for (int idx = tid; idx < mm; idx += JT) {
-    const double x = get(idx % m, idx / m) * sc;
+    const double x = ldexp(get(idx % m, idx / m), -e);  // not x * 2^-e: 2^-e overflows for e < -1023
     s = fma(x, x, s);
   }
   red[tid] = s;
@@ -90,8 +101,12 @@ __device__ double block_fro(int m, Get get, double* red) {
   }
   s = red[0];
   __syncthreads();
-  return ldexp(sqrt(s), e);
+  r = sqrt(s);
+  return true;
 }
+
+// the power s of the normalisation A^ = 4^-s A (header): floor(e / 2)
+__device__ __forceinline__ int scale_power(int e) { return e >> 1; }
 
 // Cyclic Jacobi on the symmetric np x np matrix a (np even, <= 64), accumulating the rotations into v (a @ [i + j LDJ], exactly
 // symmetric throughout).  Each step rotates the np / 2 pairs of one circle-method round at once: every thread owns whole 2 x 2
@@ -186,10 +201,19 @@ __global__ void __launch_bounds__(JT) syevj_small_kernel(int n, const double* __
     v[i + j * LDJ] = i == j ? 1.0 : 0.0;
   }
   __syncthreads();
-  const double fro = block_fro(np, [&](int i, int j) { return a[i + j * LDJ]; }, red);
-  const bool finite = fro <= DBL_MAX;
+  double r;
+  int e;
+  const bool finite = block_fro(np, [&](int i, int j) { return a[i + j * LDJ]; }, red, r, e);
+  const int sp = scale_power(e);
+  if (sp != 0) {
+    for (int idx = tid; idx < np * np; idx += JT) {
+      double& x = a[idx % np + idx / np * LDJ];
+      x = ldexp(x, -2 * sp);
+    }
+    __syncthreads();
+  }
   bool first = false, conv = false;
-  if (finite) conv = jacobi64(a, v, np, SYEVJ_U * fro, js, &first);
+  if (finite) conv = jacobi64(a, v, np, SYEVJ_U * ldexp(r, e - 2 * sp), js, &first);
   // ascending order by rank counting: rank_i = #{j : w_j < w_i or (w_j = w_i and j < i)}
   if (tid < n) {
     const double wi = a[tid + tid * LDJ];
@@ -199,7 +223,7 @@ __global__ void __launch_bounds__(JT) syevj_small_kernel(int n, const double* __
       r += (wj < wi) || (wj == wi && j < tid);
     }
     rank[tid] = r;
-    w[rank[tid]] = finite ? wi : NAN;
+    w[rank[tid]] = finite ? ldexp(wi, 2 * sp) : NAN;
   }
   __syncthreads();
   for (int idx = tid; idx < n * n; idx += JT) {
@@ -212,11 +236,11 @@ __global__ void __launch_bounds__(JT) syevj_small_kernel(int n, const double* __
 // ---- n > 64: block Jacobi -------------------------------------------------------------------------------------------------------------
 // Per matrix b of the chunk: Aw, Vt (Np x Np, ld Np; Vt = V^T, so that V[:, P] <- V[:, P] Q_P is Vt[P, :] <- Q_P^T Vt[P, :]),
 // Q (h = N / 2 tiles of 64 x 64, ld 64), quiet[h], floor, state (1 iterating, 0 converged, 2 non-finite input), dirty (some
-// subproblem rotated in this sweep).
+// subproblem rotated in this sweep), scale (the power s of A^ = 4^-s A, header).
 struct BlockJacobi {
   int n, Np;
   double *Aw, *Vt, *Q, *floor_;
-  int *quiet, *state, *dirty, *active;
+  int *quiet, *state, *dirty, *scale, *active;
 };
 
 __global__ void __launch_bounds__(JT) syevj_init_kernel(BlockJacobi bj, const double* __restrict__ A) {
@@ -226,15 +250,19 @@ __global__ void __launch_bounds__(JT) syevj_init_kernel(BlockJacobi bj, const do
   A += b * nn;
   double* Aw = bj.Aw + b * NN;
   double* Vt = bj.Vt + b * NN;
+  double r;
+  int e;
+  const bool finite = block_fro(n, [&](int i, int j) { return A[min(i, j) + (long long)max(i, j) * n]; }, red, r, e);
+  const int sp = scale_power(e);
   for (long long idx = threadIdx.x; idx < NN; idx += JT) {
     const int i = (int)(idx % Np), j = (int)(idx / Np);
-    Aw[idx] = (i < n && j < n) ? A[min(i, j) + (long long)max(i, j) * n] : 0.0;
+    Aw[idx] = (i < n && j < n) ? ldexp(A[min(i, j) + (long long)max(i, j) * n], -2 * sp) : 0.0;
     Vt[idx] = i == j ? 1.0 : 0.0;
   }
-  const double fro = block_fro(n, [&](int i, int j) { return A[min(i, j) + (long long)max(i, j) * n]; }, red);
   if (threadIdx.x == 0) {
-    bj.floor_[b] = SYEVJ_U * fro;
-    bj.state[b] = fro <= DBL_MAX ? 1 : 2;
+    bj.floor_[b] = SYEVJ_U * ldexp(r, e - 2 * sp);  // u ||A^||_F: ||A^||_F from A's own sum, which the scale-down does not change
+    bj.scale[b] = sp;
+    bj.state[b] = finite ? 1 : 2;
     bj.dirty[b] = 0;
   }
 }
@@ -370,7 +398,7 @@ __global__ void __launch_bounds__(1024) syevj_sweep_end_kernel(BlockJacobi bj, i
   if (threadIdx.x == 0) *bj.active = part[0];
 }
 
-// w = diag(A) over the real indices, sorted by rank counting; V's columns permuted alike; info = 0 converged, 1 otherwise.
+// w = 4^s diag(A^) over the real indices, sorted by rank counting; V's columns permuted alike; info = 0 converged, 1 otherwise.
 __global__ void __launch_bounds__(JT) syevj_finish_kernel(BlockJacobi bj, double* __restrict__ w, double* __restrict__ V,
                                                           int* __restrict__ info) {
   __shared__ double wv[BASECASE_MAX];
@@ -380,7 +408,7 @@ __global__ void __launch_bounds__(JT) syevj_finish_kernel(BlockJacobi bj, double
   const double* Aw = bj.Aw + b * Np * Np;
   const double* Vt = bj.Vt + b * Np * Np;
   w += b * n; V += b * n * n;
-  const int state = bj.state[b];
+  const int state = bj.state[b], sp = bj.scale[b];
   for (int i = threadIdx.x; i < n; i += JT) wv[i] = Aw[i + (long long)i * Np];
   __syncthreads();
   for (int i = threadIdx.x; i < n; i += JT) {
@@ -388,7 +416,7 @@ __global__ void __launch_bounds__(JT) syevj_finish_kernel(BlockJacobi bj, double
     int r = 0;
     for (int j = 0; j < n; j++) r += (wv[j] < wi) || (wv[j] == wi && j < i);
     rank[i] = r;
-    w[rank[i]] = state == 2 ? NAN : wi;
+    w[rank[i]] = state == 2 ? NAN : ldexp(wi, 2 * sp);
   }
   __syncthreads();
   for (long long idx = threadIdx.x; idx < (long long)n * n; idx += JT) {
@@ -437,11 +465,12 @@ capital_status_t syevj_batched(capital_ctx* ctx, cudaStream_t st, int64_t n, int
   CAP_TRY(ctx->workspace("syevj_floor", (size_t)chunk * 8, (void**)&fl));
   bj.floor_ = fl;
   int* flags;
-  CAP_TRY(ctx->workspace("syevj_flags", (size_t)(chunk * (h + 2) + 1) * sizeof(int), (void**)&flags));
+  CAP_TRY(ctx->workspace("syevj_flags", (size_t)(chunk * (h + 3) + 1) * sizeof(int), (void**)&flags));
   bj.quiet = flags;
   bj.state = flags + chunk * h;
   bj.dirty = bj.state + chunk;
-  bj.active = bj.dirty + chunk;
+  bj.scale = bj.dirty + chunk;
+  bj.active = bj.scale + chunk;
   const unsigned ntasks = (unsigned)(h * (h - 1) / 2 + (Np / 64) * h);
   for (int64_t b0 = 0; b0 < batch; b0 += chunk) {
     const int64_t cnt = std::min(chunk, batch - b0);

@@ -13,7 +13,11 @@ def syevj_batched(A: torch.Tensor, topo):
     matrix converged, 1 when it did not within the sweep bound (w and V then hold the last iterate) or when it contains NaN or Inf
     (outputs unspecified).  Nothing raises for such a matrix, and the others keep their bits.  Every matrix gets the same bits
     whatever batch it is in.  For n > 64 the call synchronises with the host once per outer sweep; for n <= 64 it is enqueued on the
-    current stream without one."""
+    current stream without one.
+
+    Each matrix is solved as 4^-s A with its largest entry in [1, 4), so every finite A is solved whatever its magnitude: an
+    eigenvalue beyond the double range comes back as +-Inf with info = 0 and an accurate V, and entries more than about 2^1074
+    below the largest one count as zero.  info = 1 means "did not converge, or holds NaN/Inf"."""
     what = "syevj_batched"
     if not isinstance(A, torch.Tensor) or A.dtype != torch.float64:
         raise ValueError(f"eig.{what}: A must be a float64 tensor")

@@ -1,10 +1,11 @@
 """A numpy model of the batched Jacobi eigensolver's exact schedule (capital_b200/csrc/syevj.cu), the test matrices with known spectra,
 and the accuracy bounds the GPU tests gate on.
 
-The model follows the kernels' decisions: the circle-method pairing, the padding of n to an even order (n <= 64) or to Np =
-roundup(n, 64) (n > 64), the skip threshold |a_pq| <= max(u sqrt|a_pp| sqrt|a_qq|, u ||A||_F), the inner sweeps on 64 x 64
+The model follows the kernels' decisions: the power-of-4 normalisation A^ = 4^-s A (s = floor(ilogb max |a_ij| / 2)), the
+circle-method pairing, the padding of n to an even order (n <= 64) or to Np =
+roundup(n, 64) (n > 64), the skip threshold |a_pq| <= max(u sqrt|a_pp| sqrt|a_qq|, u ||A^||_F), the inner sweeps on 64 x 64
 subproblems with their "quiet" flag (no rotation in the first inner sweep), the block step A <- Q^T A Q, V <- V Q over the pairs of
-one outer step, and convergence after an outer sweep in which every subproblem was quiet.  It does not model the last bits: the
+one outer step, convergence after an outer sweep in which every subproblem was quiet, and w = 4^s w^.  It does not model the last bits: the
 block update is a dense product here, and the 2 x 2 updates run as whole-row and whole-column passes."""
 import numpy as np
 
@@ -82,24 +83,42 @@ def jacobi(A, V, floor, sweeps=SWEEPS):
 
 
 def fro(a):
-    return float(np.linalg.norm(a))
+    """||a||_F summed at the scale of its largest entry, as block_fro does: finite for every finite a whose norm is below DBL_MAX"""
+    a = np.asarray(a, dtype=np.float64)
+    mx = float(np.abs(a).max()) if a.size else 0.0
+    if mx == 0.0 or not np.isfinite(mx):
+        return mx
+    e = int(np.frexp(mx)[1]) - 1
+    with np.errstate(over="ignore"):
+        return float(np.ldexp(np.linalg.norm(np.ldexp(a, -e)), e))
 
 
-def _finish(Aw, V, n):
-    """w = the real diagonal, ascending by rank counting (ties by index); V's real columns permuted alike, real rows"""
+def scale_power(a) -> int:
+    """s of the normalisation A^ = 4^-s A: floor(ilogb(max |a_ij|) / 2), 0 for a zero or non-finite matrix"""
+    mx = float(np.abs(a).max())
+    if mx == 0.0 or not np.isfinite(mx):
+        return 0
+    return (int(np.frexp(mx)[1]) - 1) // 2
+
+
+def _finish(Aw, V, n, sp):
+    """w = 4^s times the real diagonal, ascending by rank counting (ties by index); V's real columns permuted alike, real rows"""
     d = np.diagonal(Aw, axis1=1, axis2=2)[:, :n]
     order = np.argsort(d, axis=1, kind="stable")
-    w = np.take_along_axis(d, order, 1)
+    with np.errstate(over="ignore"):
+        w = np.ldexp(np.take_along_axis(d, order, 1), 2 * sp[:, None])
     Vr = np.stack([V[b][:n][:, order[b]] for b in range(V.shape[0])])
     return w, Vr
 
 
 def syevj(A, snapshots=False):
-    """The model on a batch A (B, n, n) of symmetric matrices.  Returns a dict: w, V, info, sweeps (per matrix: outer sweeps for
-    n > 64, sweeps for n <= 64), the padded iterate Aw and Vw, and for n > 64 with `snapshots`, steps: the finished (w, V) after every
+    """The model on a batch A (B, n, n) of finite symmetric matrices.  Returns a dict: w, V, info, sweeps (per matrix: outer sweeps
+    for n > 64, sweeps for n <= 64), the padded iterate Aw and Vw of the normalised matrix A^, and for n > 64 with `snapshots`, steps: the finished (w, V) after every
     outer step."""
     A = np.asarray(A, dtype=np.float64)
     B, n, _ = A.shape
+    sp = np.array([scale_power(a) for a in A])
+    A = np.ldexp(A, -2 * sp[:, None, None])
     floor = np.array([U * fro(a) for a in A])
     if n <= 64:
         m = n + (n & 1)
@@ -107,7 +126,7 @@ def syevj(A, snapshots=False):
         Aw[:, :n, :n] = A
         Vw = np.tile(np.eye(m), (B, 1, 1))
         count, _, conv = jacobi(Aw, Vw, floor)
-        w, V = _finish(Aw, Vw, n)
+        w, V = _finish(Aw, Vw, n, sp)
         return dict(w=w, V=V, info=(~conv).astype(int), sweeps=count, Aw=Aw, Vw=Vw)
     Np = -(-n // 64) * 64
     N, h = Np // 32, Np // 64
@@ -144,12 +163,12 @@ def syevj(A, snapshots=False):
                 Vw[b] = Vw[b] @ Qb
                 dirty[b] = True
             if snapshots:
-                steps.append(_finish(Aw, Vw, n))
+                steps.append(_finish(Aw, Vw, n, sp))
         sweeps += active
         active &= dirty
         if not active.any():
             break
-    w, V = _finish(Aw, Vw, n)
+    w, V = _finish(Aw, Vw, n, sp)
     return dict(w=w, V=V, info=active.astype(int), sweeps=sweeps, Aw=Aw, Vw=Vw, steps=steps)
 
 
